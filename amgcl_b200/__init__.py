@@ -1,9 +1,9 @@
-"""amgcl_b200 -- B200-native solve-phase backend for AMGCL.
+"""amgcl_b200 -- H100-native solve-phase backend for AMGCL.
 
 The product is native:
 
   include/amgcl_b200.h              C ABI (the drop-in boundary)
-  amgcl_b200/csrc/*.cu(h)           hand-written sm_100a kernels behind it
+  amgcl_b200/csrc/*.cu(h)           hand-written sm_90a kernels behind it
   include/amgcl/backend/b200.hpp    C++ binding to amgcl::backend (the reference is C++)
   amgcl_b200/host/dropin.cpp        AMGCL's own make_solver<amg<...>, cg|bicgstab>
                                     instantiated on that backend
@@ -691,7 +691,7 @@ class Graph:
 
 class DropinSolver:
     """amgcl::make_solver<amg<backend::b200<double>, smoothed_aggregation, RELAX>, KRYLOV>
-    -- the reference's own templates running on the B200 backend."""
+    -- the reference's own templates running on the H100 backend."""
 
     def __init__(self, ptr, col, val, relax="damped_jacobi", krylov="cg", tol=1e-8,
                  maxiter=100, coarse_enough=-1, ctx=None, precision="f64", graph=False):

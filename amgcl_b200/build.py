@@ -1,6 +1,6 @@
 """Build recipes for the native parts of amgcl_b200 (all in-tree, no JIT cache).
 
-  libamgcl_b200.so         CUDA kernels + C ABI (nvcc, sm_100a only; csrc/api_*.cu)
+  libamgcl_b200.so         CUDA kernels + C ABI (nvcc, sm_90a only; csrc/api_*.cu)
   libamgcl_b200_dropin.so  AMGCL's own make_solver/amg/cg/bicgstab templates
                            instantiated on backend::b200 (g++; needs the AMGCL
                            headers, i.e. only buildable where /root/reference or
@@ -25,7 +25,7 @@ EXAMPLE = os.path.join(LIBDIR, "poisson_b200")
 EXAMPLE_SRC = os.path.join(ROOT, "examples", "poisson_b200.cpp")
 
 NVCC_COMPILE = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fopenmp", "-I", INCLUDE,
 ]
@@ -70,7 +70,7 @@ def cuda_sources():
 
 
 def build_cuda(force=False, verbose=False):
-    """Compile the CUDA kernels + C ABI for sm_100a into libamgcl_b200.so (one object per
+    """Compile the CUDA kernels + C ABI for sm_90a into libamgcl_b200.so (one object per
     api_*.cu, compiled concurrently, objects kept under lib/obj/)."""
     os.makedirs(LIBDIR, exist_ok=True)
     units, headers = cuda_sources()
@@ -99,7 +99,7 @@ def build_cuda(force=False, verbose=False):
     if failed:
         raise RuntimeError("\n".join(failed))
     objs = [os.path.join(objdir, u[:-3] + ".o") for u in units]
-    _run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-Xcompiler", "-fopenmp",
+    _run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-Xcompiler", "-fopenmp",
           "-o", LIB_CUDA] + objs + ["-lgomp"])
     return LIB_CUDA
 

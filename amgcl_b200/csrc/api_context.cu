@@ -38,7 +38,7 @@ using namespace b200;
 // ---------------------------------------------------------------------------
 extern "C" const char *b200_last_error(void) { return g_last_error.c_str(); }
 
-extern "C" const char *b200_version(void) { return "amgcl_b200 0.1.0 sm_100a"; }
+extern "C" const char *b200_version(void) { return "amgcl_b200 0.1.0 sm_90a"; }
 
 extern "C" int b200_device_count(void) {
     int n = 0;
@@ -53,7 +53,9 @@ static int ctx_init(b200_ctx_t ctx, int device) {
     cudaDeviceProp prop;
     B200_CUDA(cudaGetDeviceProperties(&prop, device));
     ctx->sm_count = prop.multiProcessorCount;
-    if (prop.major < 10) return fail(B200_ECUDA, "amgcl_b200 needs an sm_100a (Blackwell B200) device");
+    // the library holds sm_90a code only, which no other compute capability can load
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(B200_ECUDA, "amgcl_b200 needs an sm_90a (Hopper H100) device");
     B200_CUDA(cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking));
     ctx->stream = ctx->own_stream;
     B200_CUDA(cudaMalloc(&ctx->dot_partial, kDotMaxBlocks * sizeof(double)));

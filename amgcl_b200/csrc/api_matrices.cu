@@ -23,9 +23,8 @@ using namespace b200;
 namespace b200 {
 
 static int choose_lanes(double avg) {
-    // measured on the B200 with the operators of a 192^3 Poisson hierarchy
-    // (tools/gpu_check.py levels): few lanes per row keep many rows -- and so many
-    // independent x-gathers -- in flight per CTA; wide groups only pay off for long rows
+    // few lanes per row keep many rows -- and so many independent x-gathers -- in flight
+    // per CTA; wide groups only pay off for long rows
     if (avg <= 12.0) return 1;
     if (avg <= 40.0) return 2;
     if (avg <= 64.0) return 4;

@@ -1,7 +1,7 @@
-// common.cuh -- shared definitions for the B200 solve-phase backend.
+// common.cuh -- shared definitions for the H100 solve-phase backend.
 //
 // Device objects behind the opaque C handles of include/amgcl_b200.h, error
-// plumbing, and the sm_100a PTX helpers (mbarrier + 1-D TMA bulk copies) the
+// plumbing, and the sm_90a PTX helpers (mbarrier + 1-D TMA bulk copies) the
 // streaming kernels are built from.
 #pragma once
 
@@ -42,7 +42,7 @@ int  cuda_fail(cudaError_t rc, const char *what, const char *file, int line);
     } while (0)
 
 // ---------------------------------------------------------------------------
-// hardware constants (B200: 148 SMs, 227 KB smem / CTA)
+// hardware constants (H100: 132 SMs, 227 KB smem / CTA)
 // ---------------------------------------------------------------------------
 constexpr int kThreads      = 256;    // threads per CTA in every streaming kernel
 constexpr int kRowsCapMax   = 1024;   // most rows a row block may hold
@@ -66,7 +66,7 @@ struct b200_graph_s;
 
 struct b200_ctx_s {
     int          device      = 0;
-    int          sm_count    = 148;
+    int          sm_count    = 132;
     cudaStream_t own_stream  = nullptr;
     cudaStream_t stream      = nullptr;   // stream in use (own or external)
     uint64_t     launches    = 0;
@@ -386,7 +386,7 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t by
 // bulk copies there, so the pipeline fill overlaps the flush.  A no-op for kernels launched
 // without the attribute.  (An explicit early griddepcontrol.launch_dependents was measured
 // and rejected: dependents that become resident early take SM resources from the running
-// persistent grid, 71.1 vs 59.7 ms per 256^3 solve; DESIGN.md section 8.)
+// persistent grid; DESIGN.md section 3.3b.)
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // streaming (read-once) 16-byte global load that does not allocate in L1

@@ -2,8 +2,8 @@
 //
 // The collectives of the partitioned solve are tiny (a halo plane, one coarse
 // vector, one scalar) and sit on the critical path ~200 times per solve, so their
-// cost is latency, not bandwidth: an NCCL call costs ~20-25 us each on B200/NVSwitch
-// (measured, profiles/r1_bench_n2_nccl_*.json).  Here every rank maps its peers'
+// cost is latency, not bandwidth: an NCCL call costs tens of microseconds each on NVSwitch.
+// Here every rank maps its peers'
 // exchange buffers once (CUDA IPC) and the data moves with plain stores from our own
 // kernels:
 //

@@ -10,7 +10,7 @@
 //
 // What makes a command cheap here:
 //   * the barrier is one red.release + a spin on ld.acquire of a monotonically increasing
-//     64-bit counter (no reset, no fences): ~1 us for 148 CTAs;
+//     64-bit counter (no reset, no fences): one per SM;
 //   * matrix data is written by nobody, so BEFORE arriving at the barrier every thread already
 //     loads the row pointers of its first row of the NEXT command and prefetches that row's
 //     first col/val lines into L1: after the barrier only the dependent x-gather is left;

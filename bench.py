@@ -1,13 +1,14 @@
 #!/usr/bin/env python
-"""bench.py -- solve-phase benchmark of the B200 backend (BASELINE.json metric).
+"""bench.py -- solve-phase benchmark of the amgcl_b200 backend on an H100 (BASELINE.json metric).
 
 Workload (config #2 of BASELINE.json): 3-D 7-point Poisson 256^3 (16.8 M unknowns,
 117 M non-zeros), FP64, AMGCL smoothed_aggregation + damped_jacobi + CG with all
 reference defaults, hierarchy built on the host by AMGCL itself, solve phase on the
-B200 through amgcl::backend::b200 (the drop-in).  One "step" = one complete solve
+GPU through amgcl::backend::b200 (the drop-in).  One "step" = one complete solve
 (rhs == 1, x0 == 0, tol 1e-8).  Metric: CG iterations per second (and solve seconds).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--n 256] [--impl b200|reference]
+                    [--dump-outputs DIR]
 
 One JSON line on stdout (rank 0).  See DESIGN.md "Measurement" for every field.
 """
@@ -32,7 +33,7 @@ UNIT = "iter/s"
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10, help="timed solves (at least 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--n", type=int, default=256, help="grid points per dimension")
@@ -53,7 +54,14 @@ def parse_args():
     ap.add_argument("--graph", type=int, default=0, choices=[0, 1],
                     help="1: amgcl::preconditioner::b200_cycle_graph<amg<...>> -- every V-cycle is one "
                          "CUDA graph launch (single GPU)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed solves, write what the last one computed (either --impl) as "
+                         "DIR/<name>.npy (float64): iters, resid and the solution x (a fixed seeded sample of it when "
+                         "it is larger than %d entries, with the sampled indices)" % DUMP_MAX_X)
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
 
 
 def workload_name(args):
@@ -67,7 +75,7 @@ def peaks():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 # --------------------------------------------------------------------------- clocks
@@ -293,8 +301,10 @@ def reference_arm(args, rank, world):
     for _ in range(args.warmup):
         Sq.solve(rhs)
     Sq.close()
-    _, it, _, secs, full, t_setup, x, it_full, res = bounded_reference_sample(
+    x_last, it, res_last, secs, full, t_setup, x, it_full, res = bounded_reference_sample(
         args, ptr, col, val, rhs, args.steps, 150.0, topo)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, x_last, it, res_last, rank)
     med = float(np.median(secs))
     value = it / med
     sample = "%d %s %s solves (%d iterations each%s), solve() only; median %.3f s, min %.3f, max %.3f" % (
@@ -325,7 +335,7 @@ def config_block(args, nrows, nnz, t_setup, t_gen, backend=None, parallelism="ho
     cfg = {"workload": workload_name(args), "rows": nrows, "nnz": nnz,
            "relax": args.relax, "krylov": args.krylov, "tol": 1e-8,
            "step": "one complete solve, rhs=1, x0=0",
-           "l2": "inputs_exceed_l2 (finest matrix %.2f GB >> 126 MB)" % (nnz * 12 / 1e9),
+           "l2": "inputs_exceed_l2 (finest matrix %.2f GB >> 50 MB)" % (nnz * 12 / 1e9),
            "parallelism": parallelism,
            "setup_s": t_setup, "generate_s": t_gen,
            "hierarchy": "host (AMGCL smoothed_aggregation)"}
@@ -382,6 +392,28 @@ def golden_parity(args, iters, resid, x):
     out["ok"] = bool(out["iters"] == out["iters_golden"] and out["resid_rel_diff"] <= 1e-6 and
                      out["x_samples_rel_err_inf"] <= 1e-8 and out["x_norm2_rel_diff"] <= 1e-8)
     return out
+
+
+DUMP_MAX_X = 4 * 1024 * 1024     # entries of x written in full; larger solutions are sampled
+
+
+def dump_outputs(out_dir, x, iters, resid, rank):
+    """What a caller of the timed path receives from its last solve: the iteration count, the
+    final relative residual and the solution.  A solution longer than DUMP_MAX_X is written as
+    the entries at DUMP_MAX_X / 2 indices drawn with a fixed seed (x_index), so two builds run
+    with the same arguments can be compared output for output; at most 64 MB in all."""
+    if rank != 0:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    out = {"iters": np.array([iters], dtype=np.float64), "resid": np.array([resid], dtype=np.float64)}
+    if x.size <= DUMP_MAX_X:
+        out["x"] = x.astype(np.float64)
+    else:
+        idx = np.sort(np.random.default_rng(0).choice(x.size, DUMP_MAX_X // 2, replace=False))
+        out["x_index"] = idx.astype(np.float64)
+        out["x"] = x[idx].astype(np.float64)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def main_arm(args, rank, world, local_rank):
@@ -458,6 +490,8 @@ def main_arm(args, rank, world, local_rank):
     iters = iters_total // args.steps
     # N > 1: ONE system, row-partitioned across the GPUs -> strong scaling
     value = iters_total / (ms * 1e-3)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, S.download_x(), it, res, rank)
 
     # ---- roofline: same K steps again with the CSR launches bracketed by events ----------
     ctx.profile_begin()
@@ -507,18 +541,6 @@ def main_arm(args, rank, world, local_rank):
                 "by_mode": {p["mode"]: {"launches": p["launches"],
                                         "GBs": alg_bytes(p) * p["launches"] / (p["total_ms"] * 1e-3) / 1e9}
                             for p in finest}}
-        # DRAM bytes per launch from the committed ncu --set full capture (only valid for the
-        # workload it was captured on: single GPU, same operator)
-        ncu = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.isfile(ncu) and world == 1:
-            try:
-                with open(ncu) as f:
-                    tj = json.load(f)
-                if int(tj.get("nnz", -1)) == nnz:
-                    roof["traffic"] = tj.get("dram_bytes_per_launch")
-                    roof["traffic_kernel"] = tj.get("kernel")
-            except Exception:
-                pass
     all_csr_ms = sum(p["total_ms"] for p in prof if p["nnz"] > 0 and p["mode"] != "coarse_gemv")
     streams = {"vec1": 2, "vec2": 3, "vec3": 4, "vec4": 5, "vec5": 6, "vec6": 7, "vec7": 8,
                "dot": 2, "relax_zero": 3, "memset": 1, "comm": 1, "coarse_tail": 1}

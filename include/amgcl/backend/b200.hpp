@@ -3,7 +3,7 @@
 
 /**
  * \file   amgcl/backend/b200.hpp
- * \brief  B200-native solve-phase backend for AMGCL (drop-in for backend::cuda).
+ * \brief  H100-native solve-phase backend for AMGCL (drop-in for backend::cuda).
  *
  * Usage is identical to the reference CUDA backend
  * (tutorial/1.poisson3Db/poisson3Db_cuda.cu:51-87):
@@ -24,7 +24,7 @@
  *
  * The header owns no numerical code: every primitive forwards to the C ABI of
  * libamgcl_b200.so (include/amgcl_b200.h), whose kernels are hand-written
- * sm_100a CUDA.  It implements the concept amgcl/backend/cuda.hpp:472-807
+ * sm_90a CUDA.  It implements the concept amgcl/backend/cuda.hpp:472-807
  * satisfies: a backend struct plus partial specialisations of the *_impl
  * customisation points of amgcl/backend/interface.hpp:191-249.  In addition
  * relaxation::damped_jacobi and relaxation::spai0 are specialised for this
@@ -268,9 +268,9 @@ class b200_dense_inverse {
 
 namespace backend {
 
-/// B200 backend.
+/// H100 backend.
 /**
- * Hand-written sm_100a kernels for every solve-phase primitive; the hierarchy
+ * Hand-written sm_90a kernels for every solve-phase primitive; the hierarchy
  * is built on the host by AMGCL's own coarsening and uploaded once.
  *
  * \param real        Value type (double).

@@ -1,5 +1,5 @@
 /*
- * amgcl_b200.h -- C ABI of the B200-native solve-phase backend for AMGCL.
+ * amgcl_b200.h -- C ABI of the H100-native solve-phase backend for AMGCL.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  Everything the AMGCL
  * solve phase asks of a backend -- amgcl::backend::{spmv, residual, vmul,
@@ -59,7 +59,7 @@ typedef struct b200_krylov_s *b200_krylov_t;  /* device-resident scalars of a Kr
 /* Thread-local message describing the last failing call. */
 const char *b200_last_error(void);
 
-/* Library version string ("amgcl_b200 <semver> sm_100a"). */
+/* Library version string ("amgcl_b200 <semver> sm_90a"). */
 const char *b200_version(void);
 
 /* Number of usable CUDA devices (0 if none: every other call will fail). */
@@ -163,7 +163,7 @@ int b200_split_info(b200_split_t sp, int64_t *nrows, int64_t *ncols, int64_t *nn
 int b200_split_copy(b200_split_t sp, int64_t *ptr, int64_t *col, double *val, int64_t *send_idx);
 int b200_split_destroy(b200_split_t sp);
 
-/* Tuning knobs (all optional; defaults are chosen for B200).
+/* Tuning knobs (all optional; defaults are chosen for the H100).
  *   "spmv_variant"     0 = one row block per CTA, 1 = persistent multi-stage ring (default)
  *   "ctas_per_sm"      persistent variant: resident CTAs per SM (default 4)
  *   "stages"           persistent variant: ring depth per CTA (default 2)
@@ -191,7 +191,7 @@ int b200_split_destroy(b200_split_t sp);
  *                      direct-load kernel instead of the TMA ring pipeline; same arithmetic,
  *                      bit-identical results.  Default 0 = always the ring kernel: measured, the
  *                      ring kernel wins even on tiny operators because its first bulk copies
- *                      are issued before the grid dependency resolves (64^3: 1.40 vs 1.60 ms)
+ *                      are issued before the grid dependency resolves
  *   "poll_scalars"     1 = a host-synchronous result of an in-kernel reduction (b200_dot, the
  *                      Krylov steps) is awaited by polling the mapped host word the finishing CTA
  *                      releases (default), 0 = by cudaStreamSynchronize
@@ -310,7 +310,7 @@ int b200_csr_offsets(b200_csr_t A, int *offset_indexed, int *count);
 int b200_offset_plan_i64(int64_t nrows, int64_t ncols, const int64_t *ptr, const int64_t *col,
                          uint8_t *idx8_out, int32_t *tab_out, int *count, int *qualifies);
 
-/* Windowed operators (opt-in: measured slower than the plain path on B200, DESIGN.md).  An
+/* Windowed operators (opt-in: measured slower than the plain path, DESIGN.md).  An
  * operator whose row blocks gather x from few contiguous places
  * (the level matrices and prolongations of a structured problem) is additionally stored with
  * 16-bit window-local columns plus, per row block, the runs of x its window is made of; the

@@ -2,7 +2,7 @@
  * amg_oracle.c -- TEST INFRASTRUCTURE, never shipped, never on the product path.
  *
  * A plain-C, single-threaded restatement of the AMGCL solve phase that the
- * B200 backend accelerates.  Only tests/, __graft_entry__.smoke() and
+ * H100 backend accelerates.  Only tests/, __graft_entry__.smoke() and
  * bench.py's cpu_baseline leg may load this file's library.  Each function
  * cites the reference code (paths relative to /root/reference) it restates.
  *

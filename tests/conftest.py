@@ -19,7 +19,7 @@ TOL_SOLUTION = 1e-8        # ||x - x_ref||_inf / ||x_ref||_inf after a converged
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def _have_gpu():
