@@ -43,6 +43,15 @@ class ProfileEntry(_c.Structure):
                 ("launches", _i64), ("total_ms", _dbl), ("min_ms", _dbl)]
 
 
+class ProfileFormatEntry(_c.Structure):
+    """b200_profile_format_entry (include/amgcl_b200_formats.h)."""
+    _fields_ = [("entry", ProfileEntry), ("format", _c.c_int)]
+
+
+# column formats of a CSR operator (include/amgcl_b200_formats.h B200_FMT_*)
+FORMAT_NAMES = ("plain", "window", "offset", "pattern", "col16", "col24")
+
+
 # vecK: element-wise pass over K+1 vector streams (reads + writes)
 MODE_NAMES = {0: "spmv", 1: "spmv_acc", 2: "residual", 3: "relax", 4: "residual_scaled", 10: "vec1", 11: "vec2",
               12: "vec3", 13: "vec4", 14: "vec5", 15: "vec6", 16: "vec7",
@@ -137,6 +146,9 @@ def lib():
         "b200_pattern_plan_i64": [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _P(_c.c_int), _P(_c.c_int), _P(_c.c_int)],
         "b200_csr_offsets": [_vp, _P(_c.c_int), _P(_c.c_int)],
         "b200_offset_plan_i64": [_i64, _i64, _vp, _vp, _vp, _vp, _P(_c.c_int), _P(_c.c_int)],
+        "b200_csr_narrow": [_vp, _P(_c.c_int)],
+        "b200_narrow_plan_i64": [_i64, _i64, _vp, _vp, _c.c_int, _c.c_int, _vp, _i64, _vp, _vp, _vp,
+                                 _P(_i64), _P(_c.c_int)],
         "b200_csr_window": [_vp, _P(_c.c_int), _P(_c.c_int), _P(_c.c_int), _P(_i64)],
         "b200_window_plan_i64": [_i64, _i64, _vp, _vp, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _c.c_int, _vp, _vp, _i64,
                                  _vp, _i64, _P(_i64), _P(_i64), _P(_c.c_int), _P(_c.c_int), _P(_c.c_int)],
@@ -165,6 +177,7 @@ def lib():
         "b200_bicg_step_r": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _P(_dbl), _P(_dbl)],
         "b200_profile_begin": [_vp],
         "b200_profile_end": [_vp, _vp, _i64, _P(_i64)],
+        "b200_profile_end_formats": [_vp, _vp, _i64, _P(_i64)],
     }
     for name, args in sigs.items():
         fn = getattr(L, name)
@@ -305,26 +318,27 @@ class Context:
 
     def largest_operator(self):
         """(non-zeros, column format) of the largest operator uploaded so far; format is one of
-        'plain', 'window', 'offset', 'pattern'."""
+        one of FORMAT_NAMES."""
         nnz, fmt = _i64(), _c.c_int()
         _check(lib().b200_ctx_largest_operator(self.h, _c.byref(nnz), _c.byref(fmt)))
-        return nnz.value, ("plain", "window", "offset", "pattern")[fmt.value]
+        return nnz.value, FORMAT_NAMES[fmt.value]
 
     def profile_begin(self):
         _check(lib().b200_profile_begin(self.h), "b200_profile_begin")
 
     def profile_end(self):
-        """Per (matrix shape, mode) device times of the CSR kernels since profile_begin()."""
+        """Per (matrix shape, mode, column format) device times of the CSR kernels since
+        profile_begin()."""
         cap = 256
-        buf = (ProfileEntry * cap)()
+        buf = (ProfileFormatEntry * cap)()
         cnt = _i64()
-        _check(lib().b200_profile_end(self.h, buf, cap, _c.byref(cnt)), "b200_profile_end")
+        _check(lib().b200_profile_end_formats(self.h, buf, cap, _c.byref(cnt)), "b200_profile_end_formats")
         out = []
         for i in range(min(cap, cnt.value)):
-            e = buf[i]
+            e, fmt = buf[i].entry, buf[i].format
             out.append({"nrows": e.nrows, "ncols": e.ncols, "nnz": e.nnz,
                         "mode": MODE_NAMES.get(e.mode, str(e.mode)), "launches": e.launches,
-                        "total_ms": e.total_ms, "min_ms": e.min_ms})
+                        "total_ms": e.total_ms, "min_ms": e.min_ms, "format": FORMAT_NAMES[fmt]})
         return out
 
     def close(self):
@@ -546,6 +560,13 @@ class Csr:
         _check(lib().b200_csr_offsets(self.h, _c.byref(on), _c.byref(cnt)))
         return {"offset_indexed": bool(on.value), "count": cnt.value}
 
+    def narrow(self):
+        """Width of this operator's block-relative columns: 16, 24, or 0 when it is not stored
+        that way (b200_csr_narrow)."""
+        w = _c.c_int()
+        _check(lib().b200_csr_narrow(self.h, _c.byref(w)))
+        return w.value
+
     def window(self):
         """Windowed storage of this operator (include/amgcl_b200.h: b200_csr_window)."""
         w, ms, mr, tot = _c.c_int(), _c.c_int(), _c.c_int(), _i64()
@@ -591,6 +612,31 @@ def offset_plan(nrows, ncols, ptr, col):
     if not ok.value:
         return None
     return {"idx8": idx8[:nnz], "tab": tab, "count": cnt.value}
+
+
+def narrow_plan(nrows, ncols, ptr, col, lanes=0, nnz_cap=2048):
+    """Host-only: the row-block plan's block-relative row pointers and narrow columns
+    b200_csr_create would build for a single-GPU operator (b200_narrow_plan_i64).  A dict with
+    nblocks, ptr16 [nrows] and width (16, 24, or 0 when the operator stays plain); when narrowed
+    also base [nblocks], lo16 [nnz] and, width 24, hi8 [nnz]."""
+    ptr = np.ascontiguousarray(ptr, dtype=np.int64)
+    col = np.ascontiguousarray(col, dtype=np.int64)
+    nnz = int(ptr[-1]) if nrows else 0
+    cap = nrows // 4 + 2 + (nnz // 256 + 1)        # at least one block per quad or per 256 entries
+    base = np.zeros(cap, dtype=np.int32)
+    lo16 = np.zeros(max(1, nnz), dtype=np.uint16)
+    hi8 = np.zeros(max(1, nnz), dtype=np.uint8)
+    ptr16 = np.zeros(max(1, nrows), dtype=np.uint16)
+    nb, w = _i64(), _c.c_int()
+    _check(lib().b200_narrow_plan_i64(nrows, ncols, ptr.ctypes.data, col.ctypes.data, int(lanes), int(nnz_cap),
+                                      base.ctypes.data, cap, lo16.ctypes.data, hi8.ctypes.data,
+                                      ptr16.ctypes.data, _c.byref(nb), _c.byref(w)))
+    out = {"nblocks": nb.value, "ptr16": ptr16[:nrows], "width": w.value}
+    if w.value:
+        out.update(base=base[:nb.value], lo16=lo16[:nnz])
+        if w.value == 24:
+            out["hi8"] = hi8[:nnz]
+    return out
 
 
 def window_plan(nrows, ncols, ptr, col, lanes=0, nnz_cap=2048, slot_cap=1400, max_ratio=75, gap=2):

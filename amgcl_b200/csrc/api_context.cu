@@ -91,6 +91,7 @@ extern "C" int b200_ctx_create(int device, b200_ctx_t *out) {
     if (const char *e = getenv("B200_PATTERNS_MIN_NNZ")) ctx->opt_patterns_min_nnz = atoll(e);
     if (const char *e = getenv("B200_OFFSETS")) ctx->opt_offsets = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_OFFSETS_MIN_NNZ")) ctx->opt_offsets_min_nnz = atoll(e);
+    if (const char *e = getenv("B200_NARROW_COLUMNS")) ctx->opt_narrow = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_WINDOW")) ctx->opt_window = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_WINDOW_MIN_NNZ")) ctx->opt_window_min_nnz = atoll(e);
     if (const char *e = getenv("B200_WINDOW_GAP")) ctx->opt_window_gap = std::max(1, std::min(8, atoi(e)));
@@ -225,33 +226,56 @@ extern "C" int b200_profile_begin(b200_ctx_t ctx) {
     return B200_OK;
 }
 
-extern "C" int b200_profile_end(b200_ctx_t ctx, b200_profile_entry *out, int64_t capacity,
-                                int64_t *count) {
-    CHECK_CTX(ctx);
-    B200_REQUIRE(count != nullptr, "null output pointer");
+// per (shape, mode, format) device times of the launches since b200_profile_begin
+static int profile_collect(b200_ctx_t ctx, std::vector<b200_profile_format_entry> &agg) {
     GUARD(ctx);
     ctx->profiling = false;
     B200_CUDA(cudaStreamSynchronize(ctx->stream));
-    std::vector<b200_profile_entry> agg;
     for (const auto &r : ctx->prof_recs) {
         float ms = 0.f;
         B200_CUDA(cudaEventElapsedTime(&ms, ctx->prof_events[r.ev], ctx->prof_events[r.ev + 1]));
-        b200_profile_entry *hit = nullptr;
+        b200_profile_format_entry *hit = nullptr;
         for (auto &a : agg)
-            if (a.nrows == r.nrows && a.ncols == r.ncols && a.nnz == r.nnz && a.mode == r.mode) {
+            if (a.entry.nrows == r.nrows && a.entry.ncols == r.ncols && a.entry.nnz == r.nnz &&
+                a.entry.mode == r.mode && a.format == r.fmt) {
                 hit = &a;
                 break;
             }
         if (!hit) {
-            agg.push_back({r.nrows, r.ncols, r.nnz, r.mode, 0, 0.0, 1e30});
+            agg.push_back({{r.nrows, r.ncols, r.nnz, r.mode, 0, 0.0, 1e30}, r.fmt});
             hit = &agg.back();
         }
-        hit->launches += 1;
-        hit->total_ms += ms;
-        if (ms < hit->min_ms) hit->min_ms = ms;
+        hit->entry.launches += 1;
+        hit->entry.total_ms += ms;
+        if (ms < hit->entry.min_ms) hit->entry.min_ms = ms;
     }
     ctx->prof_recs.clear();
     ctx->prof_used = 0;
+    return B200_OK;
+}
+
+extern "C" int b200_profile_end(b200_ctx_t ctx, b200_profile_entry *out, int64_t capacity,
+                                int64_t *count) {
+    CHECK_CTX(ctx);
+    B200_REQUIRE(count != nullptr, "null output pointer");
+    std::vector<b200_profile_format_entry> agg;
+    const int rc = profile_collect(ctx, agg);
+    if (rc) return rc;
+    *count = (int64_t)agg.size();
+    if (out) {
+        const int64_t m = std::min<int64_t>(capacity, (int64_t)agg.size());
+        for (int64_t i = 0; i < m; ++i) out[i] = agg[(size_t)i].entry;
+    }
+    return B200_OK;
+}
+
+extern "C" int b200_profile_end_formats(b200_ctx_t ctx, b200_profile_format_entry *out, int64_t capacity,
+                                        int64_t *count) {
+    CHECK_CTX(ctx);
+    B200_REQUIRE(count != nullptr, "null output pointer");
+    std::vector<b200_profile_format_entry> agg;
+    const int rc = profile_collect(ctx, agg);
+    if (rc) return rc;
     *count = (int64_t)agg.size();
     if (out) {
         const int64_t m = std::min<int64_t>(capacity, (int64_t)agg.size());
@@ -283,6 +307,7 @@ static int64_t *option_slot(b200_ctx_t ctx, const char *key) {
     if (!strcmp(key, "patterns_min_nnz")) return &ctx->opt_patterns_min_nnz;
     if (!strcmp(key, "offsets")) return &ctx->opt_offsets;
     if (!strcmp(key, "offsets_min_nnz")) return &ctx->opt_offsets_min_nnz;
+    if (!strcmp(key, "narrow_columns")) return &ctx->opt_narrow;
     if (!strcmp(key, "window")) return &ctx->opt_window;
     if (!strcmp(key, "window_min_nnz")) return &ctx->opt_window_min_nnz;
     if (!strcmp(key, "window_ratio")) return &ctx->opt_window_ratio;

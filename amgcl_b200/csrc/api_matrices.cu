@@ -8,6 +8,7 @@
 #include "window.cuh"
 #include "offsets.cuh"
 #include "patterns.cuh"
+#include "narrow.cuh"
 
 namespace b200 {
 int tail_enqueue_csr(b200_ctx_t ctx, int mode, b200_csr_t A, const CsrArgsT<PrecDD> &a);   // api_tail.cu
@@ -215,6 +216,15 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
         }
     }
 
+    // ---- narrow columns for the operators no other format takes (narrow.cuh) -----------------
+    NarrowPlan nar;
+    const bool narrowed = !pattern_indexed && !offset_indexed && !windowed && ctx->opt_narrow && nlong == 0 &&
+                          lanes <= 8 && build_narrow(blk4.data(), nblocks, col, nnz, nar);
+
+    // ---- block-relative row pointers of the final blocks --------------------------------
+    std::vector<unsigned short> ptr16((size_t)nrows, 0);
+    build_ptr16(blk4.data(), nblocks, hptr.data(), nnz_cap, ptr16);
+
     // ---- upload ---------------------------------------------------------------------
     b200_csr_s *A = new (std::nothrow) b200_csr_s();
     if (!A) return fail(B200_ENOMEM, "out of host memory");
@@ -235,6 +245,10 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     const size_t tab_bytes = offset_indexed ? kOffTabLen * sizeof(int) : 0;
     const size_t pid_bytes = pattern_indexed ? (((size_t)nrows + 32 + 15) & ~(size_t)15) : 0;
     const size_t pat_bytes = pattern_indexed ? kPatOffCap * sizeof(int) + (kPatCap + 1 + 7) * sizeof(unsigned short) : 0;
+    const size_t p16_bytes = ((size_t)nrows + 16) * sizeof(unsigned short);
+    const size_t lo_bytes  = narrowed ? ((size_t)nnz + 16) * sizeof(unsigned short) : 0;
+    const size_t hi_bytes  = narrowed && nar.width == 24 ? (((size_t)nnz + 32 + 15) & ~(size_t)15) : 0;
+    const size_t cb_bytes  = narrowed ? ((size_t)nblocks + 1) * sizeof(int) : 0;
     auto cleanup = [&]() {
         if (A->ptr) cudaFree(A->ptr);
         if (A->col) cudaFree(A->col);
@@ -248,6 +262,10 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
         if (A->pid) cudaFree(A->pid);
         if (A->pat_start) cudaFree(A->pat_start);
         if (A->pat_off) cudaFree(A->pat_off);
+        if (A->ptr16) cudaFree(A->ptr16);
+        if (A->clo16) cudaFree(A->clo16);
+        if (A->chi8) cudaFree(A->chi8);
+        if (A->cbase) cudaFree(A->cbase);
         delete A;
     };
 #define CSR_CUDA(call)                                                         \
@@ -271,6 +289,23 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
         CSR_CUDA(staged_upload(ctx, static_cast<Val *>(A->val), val, (size_t)nnz));
     }
     CSR_CUDA(cudaMemcpyAsync(A->blk, blk4.data(), blk_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    CSR_CUDA(cudaMalloc(&A->ptr16, p16_bytes));
+    CSR_CUDA(cudaMemsetAsync(A->ptr16, 0, p16_bytes, ctx->stream));
+    if (nrows) CSR_CUDA(staged_upload(ctx, A->ptr16, ptr16.data(), (size_t)nrows));
+    if (narrowed) {
+        CSR_CUDA(cudaMalloc(&A->clo16, lo_bytes));
+        CSR_CUDA(cudaMalloc(&A->cbase, cb_bytes));
+        CSR_CUDA(cudaMemsetAsync(A->clo16, 0, lo_bytes, ctx->stream));
+        CSR_CUDA(cudaMemsetAsync(A->cbase, 0, cb_bytes, ctx->stream));
+        CSR_CUDA(staged_upload(ctx, A->clo16, nar.lo16.data(), (size_t)nnz));
+        CSR_CUDA(staged_upload(ctx, A->cbase, nar.base.data(), (size_t)nblocks));
+        if (nar.width == 24) {
+            CSR_CUDA(cudaMalloc(&A->chi8, hi_bytes));
+            CSR_CUDA(cudaMemsetAsync(A->chi8, 0, hi_bytes, ctx->stream));
+            CSR_CUDA(staged_upload(ctx, A->chi8, nar.hi8.data(), (size_t)nnz));
+        }
+        A->narrow = nar.width;
+    }
     if (windowed) {
         CSR_CUDA(cudaMalloc(&A->col16, c16_bytes));
         CSR_CUDA(cudaMalloc(&A->wrun, run_bytes));
@@ -307,10 +342,10 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     CSR_CUDA(cudaStreamSynchronize(ctx->stream));   // host staging buffers die here
 #undef CSR_CUDA
     A->bytes = ptr_bytes + col_bytes + val_bytes + blk_bytes + c16_bytes + run_bytes + wbk_bytes + ix8_bytes +
-               tab_bytes + pid_bytes + pat_bytes;
+               tab_bytes + pid_bytes + pat_bytes + p16_bytes + lo_bytes + hi_bytes + cb_bytes;
     if (nnz > ctx->big_nnz) {
         ctx->big_nnz = nnz;
-        ctx->big_fmt = pattern_indexed ? FMT_PATTERN : offset_indexed ? FMT_OFFSET : windowed ? FMT_WINDOW : FMT_PLAIN;
+        ctx->big_fmt = stored_format(A);
     }
     *out = A;
     if (halo_from < 0 && !windowed && ctx->opt_warm_lines && lanes >= 2 && A->dtype == B200_F64 && nblocks > 0 &&
@@ -370,6 +405,10 @@ static void csr_free(b200_csr_t A) {
     if (A->pid) cudaFree(A->pid);
     if (A->pat_start) cudaFree(A->pat_start);
     if (A->pat_off) cudaFree(A->pat_off);
+    if (A->ptr16) cudaFree(A->ptr16);
+    if (A->clo16) cudaFree(A->clo16);
+    if (A->chi8) cudaFree(A->chi8);
+    if (A->cbase) cudaFree(A->cbase);
     if (A->send_idx) cudaFree(A->send_idx);
     if (A->halo_owned) cudaFree(A->halo_owned);
     if (A->ybuf) cudaFree(A->ybuf);
@@ -519,6 +558,14 @@ static int launch_csr_LH(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) 
                 rc = launch_ring_win<MODE, L, HALO, P>(ctx, A, args);
                 done = true;
             }
+            if (fmt == FMT_COL16) {
+                rc = launch_ring_c16<MODE, L, HALO, P>(ctx, A, args);
+                done = true;
+            }
+            if (fmt == FMT_COL24) {
+                rc = launch_ring_c24<MODE, L, HALO, P>(ctx, A, args);
+                done = true;
+            }
         }
         if (!done) rc = launch_ring_impl<MODE, L, HALO, P, FMT_PLAIN>(ctx, A, args);
         if (rc) return rc;
@@ -550,7 +597,7 @@ static int launch_csr(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {
         !args.gather_on && small_csr_accepts(ctx, A))
         return small_csr_launch(ctx, MODE, A, *reinterpret_cast<const CsrArgsT<PrecDD> *>(&args));
     if (ctx->recording) A->in_graph = true;
-    ProfScope prof(ctx, MODE, A->nrows, A->ncols, A->nnz);
+    ProfScope prof(ctx, MODE, A->nrows, A->ncols, A->nnz, launch_format<P>(ctx, A));
     switch (A->lanes) {
     case 1:  return launch_csr_L<MODE, 1>(ctx, A, args);
     case 2:  return launch_csr_L<MODE, 2>(ctx, A, args);
@@ -565,13 +612,14 @@ template <class P>
 static CsrArgsT<P> base_args_t(b200_csr_t A) {
     CsrArgsT<P> a;
     memset(&a, 0, sizeof(a));
-    a.ptr = A->ptr; a.col = A->col; a.val = static_cast<const typename P::TV *>(A->val); a.blk = A->blk;
+    a.ptr = A->ptr; a.ptr16 = A->ptr16; a.col = A->col; a.val = static_cast<const typename P::TV *>(A->val); a.blk = A->blk;
     a.nrows = (int)A->nrows; a.nblocks = (int)A->nblocks;
     a.rows_cap = A->rows_cap; a.nnz_cap = A->nnz_cap;
     if (std::is_same<P, PrecDD>::value && A->ctx->opt_warm_lines) { a.wl_ptr = A->wl_ptr; a.wl = A->wl; }
     a.col16 = A->col16; a.wrun = A->wrun; a.wblk = A->wblk; a.run_cap = A->win_runs;
     a.idx8 = A->idx8; a.off_tab = A->off_tab;
     a.pid = A->pid; a.pat_start = A->pat_start; a.pat_off = A->pat_off; a.pat_total = A->pat_total;
+    a.clo16 = A->clo16; a.chi8 = A->chi8; a.cbase = A->cbase;
     return a;
 }
 static CsrArgs base_args(b200_csr_t A) { return base_args_t<PrecDD>(A); }
@@ -745,6 +793,47 @@ extern "C" int b200_pattern_plan_i64(int64_t nrows, int64_t ncols, const int64_t
     return B200_OK;
 }
 
+// The narrow column format of a host matrix (narrow.cuh), for tests: the same plan csr_upload
+// builds, without a device.  width_out: 16, 24, or 0 when the operator stays plain (a column span
+// beyond 24 bits or a long block); ptr16_out: the block-relative row pointers of that plan.
+extern "C" int b200_narrow_plan_i64(int64_t nrows, int64_t ncols, const int64_t *ptr, const int64_t *col,
+                                    int lanes, int nnz_cap, int32_t *base_out, int64_t base_capacity,
+                                    uint16_t *lo16_out, uint8_t *hi8_out, uint16_t *ptr16_out,
+                                    int64_t *nblocks_out, int *width_out) {
+    B200_REQUIRE(nrows >= 0 && ncols >= 0 && ptr && nblocks_out && width_out, "bad argument");
+    B200_REQUIRE(nnz_cap >= 256 && nnz_cap <= kNnzCapMax && nnz_cap % 8 == 0, "bad nnz_cap");
+    B200_REQUIRE(lanes == 0 || (lanes >= 1 && lanes <= 32 && !(lanes & (lanes - 1))), "bad lanes");
+    int rc = csr_validate(nrows, ncols, ptr, col, true);
+    if (rc) return rc;
+    RowBlockPlan plan;
+    build_plan(nrows, ptr, lanes, nnz_cap, plan);
+    const int64_t nblocks = (int64_t)plan.blk.size() - 1;
+    std::vector<int4> blk4((size_t)nblocks + 1);
+    for (int64_t b = 0; b < nblocks; ++b)
+        blk4[(size_t)b] = make_int4(plan.blk[(size_t)b].x, plan.blk[(size_t)b + 1].x, plan.blk[(size_t)b].y,
+                                    plan.blk[(size_t)b + 1].y);
+    const int64_t nnz = nrows ? ptr[nrows] : 0;
+    std::vector<int32_t> hptr((size_t)nrows + 1);
+    for (int64_t i = 0; i <= nrows; ++i) hptr[(size_t)i] = (int32_t)ptr[i];
+    *nblocks_out = nblocks;
+    if (ptr16_out) {
+        std::vector<unsigned short> p16((size_t)nrows, 0);
+        build_ptr16(blk4.data(), nblocks, hptr.data(), nnz_cap, p16);
+        std::copy(p16.begin(), p16.end(), ptr16_out);
+    }
+    NarrowPlan o;
+    const bool ok = plan.nlong == 0 && plan.lanes <= 8 && build_narrow(blk4.data(), nblocks, col, nnz, o);
+    *width_out = ok ? o.width : 0;
+    if (!ok) return B200_OK;
+    if (base_out) {
+        B200_REQUIRE(base_capacity >= nblocks, "block output buffer too small");
+        std::copy(o.base.begin(), o.base.end(), base_out);
+    }
+    if (lo16_out) std::copy(o.lo16.begin(), o.lo16.end(), lo16_out);
+    if (hi8_out && o.width == 24) std::copy(o.hi8.begin(), o.hi8.end(), hi8_out);
+    return B200_OK;
+}
+
 extern "C" int b200_ctx_largest_operator(b200_ctx_t ctx, int64_t *nnz, int *format) {
     CHECK_CTX(ctx);
     if (nnz) *nnz = ctx->big_nnz;
@@ -764,6 +853,12 @@ extern "C" int b200_csr_offsets(b200_csr_t A, int *offset_indexed, int *count) {
     B200_REQUIRE(A, "null argument");
     if (offset_indexed) *offset_indexed = A->idx8 ? 1 : 0;
     if (count) *count = A->off_count;
+    return B200_OK;
+}
+
+extern "C" int b200_csr_narrow(b200_csr_t A, int *width) {
+    B200_REQUIRE(A && width, "null argument");
+    *width = A->narrow;
     return B200_OK;
 }
 

@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "../../include/amgcl_b200.h"
+#include "../../include/amgcl_b200_formats.h"
 
 namespace b200 {
 
@@ -121,7 +122,7 @@ struct b200_ctx_s {
     bool                      profiling = false;
     std::vector<cudaEvent_t>  prof_events;      // pool, used pairwise
     size_t                    prof_used = 0;
-    struct ProfRec { int64_t nrows, ncols, nnz; int mode; size_t ev; };
+    struct ProfRec { int64_t nrows, ncols, nnz; int mode; size_t ev; int fmt; };
     std::vector<ProfRec>      prof_recs;
 
     // multi-GPU (dist.cuh): one process per GPU, this context's share of the job
@@ -163,6 +164,7 @@ struct b200_ctx_s {
     int64_t opt_patterns_min_nnz = 1000000;// ... from this many non-zeros on (decided at upload)
     int64_t opt_offsets       = 1;        // operators with <= 256 distinct (col - row): 8-bit column indices
     int64_t opt_offsets_min_nnz = 1000000;// ... from this many non-zeros on (decided at upload)
+    int64_t opt_narrow        = 1;        // other operators: 16- or 24-bit block-relative columns (narrow.cuh)
     int64_t opt_window        = 0;        // operators that qualify gather x through shared-memory windows
     int64_t opt_window_min_nnz = 1000000; // ... "qualify": at least this many non-zeros (decided at upload),
     int64_t opt_window_ratio  = 75;       // ... windows no larger than this percentage of the entries,
@@ -277,6 +279,13 @@ struct b200_csr_s {
     unsigned short *pat_start = nullptr;  // [257] device
     int            *pat_off   = nullptr;  // [1024] device
     int        pat_count = 0, pat_total = 0;
+    // block-relative row pointers of every staged format: ptr16[r] = ptr[r] - first non-zero of r's block
+    unsigned short *ptr16 = nullptr;  // [nrows] (+ padding)
+    // block-relative columns (narrow.cuh): col = cbase[block] + clo16 (+ chi8 << 16)
+    int        narrow   = 0;          // 16 / 24: width of the stored columns; 0: not narrowed
+    unsigned short *clo16 = nullptr;  // [nnz] (+ padding) low 16 bits of col - base
+    unsigned char  *chi8  = nullptr;  // [nnz] (+ padding) high 8 bits (width 24 only)
+    int       *cbase    = nullptr;    // [nblocks] walk order: smallest column of the block
     int4      *blk      = nullptr;// [nblocks] device, walk order: {first row (~r if the block gathers halo
                                   //   columns), end row, first nnz, end nnz}; HALO: interior blocks first
     size_t     bytes    = 0;

@@ -11,8 +11,8 @@
 // Data movement.  The matrix is cut (on the host, once, at upload) into row
 // blocks: runs of consecutive rows starting at a multiple of four whose
 // non-zeros fit a shared-memory stage.  A block's slice of `val`, `col` and
-// `ptr` is contiguous in global memory, so one elected thread fetches it with
-// three 1-D TMA bulk copies (cp.async.bulk -> SASS UBLKCP) that complete on an
+// `ptr16` (row pointers relative to the block's first non-zero) is contiguous in
+// global memory, so one elected thread fetches it with one 1-D TMA bulk copy each (cp.async.bulk -> SASS UBLKCP) that complete on an
 // mbarrier; the matrix stream never passes through registers and is tagged
 // L2::evict_first so it does not displace the gathered x-vector.  Rows are
 // then reduced out of shared memory by groups of L lanes (L = 1..32, chosen
@@ -54,6 +54,11 @@
 // shared-memory load per entry, as many as the plain path needs for its staged column.  The
 // default for every operator that qualifies (the finest level of a structured-grid problem).
 //
+// Narrow columns (FMT_COL16 / FMT_COL24).  Every other operator (no long blocks, <= 8 lanes per
+// row) stores, per block, its smallest column and, per entry, the low 16 bits of col - base, plus
+// the high 8 bits in an array of their own where some block spans more than 16 bits
+// (narrow.cuh): 2 or 3 instead of 4 bytes of column per entry.
+//
 // Between blocks the CTA synchronises with a barrier (plain, windowed) or not at all
 // (offset- / pattern-indexed: the last warp done with a stage refills it) -- see the ring kernel.
 //
@@ -75,7 +80,12 @@ namespace b200 {
 enum { FMT_PLAIN = 0,     // int32 column per entry
        FMT_WINDOW = 1,    // 16-bit position in the block's shared-memory window of x
        FMT_OFFSET = 2,    // 8-bit index into a table of (col - row) offsets
-       FMT_PATTERN = 3 }; // no per-entry column: 8-bit pattern id per row, col = row + pattern[k]
+       FMT_PATTERN = 3,   // no per-entry column: 8-bit pattern id per row, col = row + pattern[k]
+       FMT_COL16 = 4,     // 16-bit column relative to the block's smallest column
+       FMT_COL24 = 5 };   // the same in 24 bits: a 16-bit and an 8-bit array
+static_assert(FMT_PLAIN == B200_FMT_PLAIN && FMT_WINDOW == B200_FMT_WINDOW && FMT_OFFSET == B200_FMT_OFFSET &&
+              FMT_PATTERN == B200_FMT_PATTERN && FMT_COL16 == B200_FMT_COL16 && FMT_COL24 == B200_FMT_COL24,
+              "formats as include/amgcl_b200_formats.h reports them");
 
 enum { MODE_SPMV = 0, MODE_SPMV_ACC = 1, MODE_RESID = 2, MODE_RELAX = 3,
        // y = f - A x with x = (alpha*d).*f formed on the fly and written to xw: the smoother's
@@ -104,7 +114,8 @@ typedef Prec<float, float, float, double, float>     PrecFFD;  // prolongation i
 
 template <class P>
 struct CsrArgsT {
-    const int    *ptr;
+    const int    *ptr;    // (long blocks)
+    const unsigned short *ptr16;   // staged blocks: ptr[r] - first non-zero of r's block
     const int    *col;
     const typename P::TV *val;
     const int4   *blk;    // [nblocks] in WALK ORDER: {first row (~first row if the block gathers
@@ -162,6 +173,10 @@ struct CsrArgsT {
     const unsigned short *pat_start;
     const int    *pat_off;
     int           pat_total;   // entries of pat_off in use (<= kPatOffCap)
+    // Narrow columns (FMT_COL16 / FMT_COL24): col = cbase[block] + clo16[e] (+ chi8[e] << 16)
+    const unsigned short *clo16;
+    const unsigned char  *chi8;
+    const int    *cbase;  // [nblocks] in walk order
     typename P::TY       *y;      // output
     typename P::TX       *xw;     // RESID_SCALED: where x = (alpha*d).*f is written
     const typename P::TF *f;      // rhs          (RESID, RELAX)
@@ -179,7 +194,7 @@ typedef CsrArgsT<PrecDD> CsrArgs;
 
 // ---- shared memory layout of one stage --------------------------------------
 struct StageLayout {
-    int val_off, col_off, ptr_off, run_off, pid_off, bytes;
+    int val_off, col_off, hi_off, ptr_off, run_off, pid_off, bytes;
 };
 // fmt: storage format of the columns (FMT_*); run_cap: FMT_WINDOW only, most runs a block has
 __host__ __device__ inline StageLayout stage_layout(int rows_cap, int nnz_cap, int val_size,
@@ -189,13 +204,17 @@ __host__ __device__ inline StageLayout stage_layout(int rows_cap, int nnz_cap, i
     int val_bytes = nnz_cap * val_size + 16;       // source aligned down to 16 B
     val_bytes = (val_bytes + 15) & ~15;
     s.col_off = s.val_off + val_bytes;
-    int col_bytes = fmt == FMT_WINDOW  ? (nnz_cap + 16) * 2   // +7 align down, +7 round up
+    const bool narrow = fmt == FMT_COL16 || fmt == FMT_COL24;
+    int col_bytes = fmt == FMT_WINDOW || narrow ? (nnz_cap + 16) * 2   // +7 align down, +7 round up
                   : fmt == FMT_OFFSET  ? (nnz_cap + 32)       // +15 align down, +15 round up
                   : fmt == FMT_PATTERN ? 0
                                        : (nnz_cap + 8) * 4;   // +3 align down, +3 round up
     col_bytes = (col_bytes + 15) & ~15;
-    s.ptr_off = s.col_off + col_bytes;
-    int ptr_bytes = (rows_cap + 4) * 4;
+    s.hi_off = s.col_off + col_bytes;
+    int hi_bytes = fmt == FMT_COL24 ? nnz_cap + 32 : 0;       // +15 align down, +15 round up
+    hi_bytes = (hi_bytes + 15) & ~15;
+    s.ptr_off = s.hi_off + hi_bytes;
+    int ptr_bytes = (rows_cap + 16) * 2;                      // 16-bit: +7 align down, +7 round up
     ptr_bytes = (ptr_bytes + 15) & ~15;
     s.run_off = s.ptr_off + ptr_bytes;
     int run_bytes = fmt == FMT_WINDOW ? (run_cap + 2) * 8 : 0;   // +1 align down, +1 round up
@@ -221,7 +240,7 @@ struct BlockDesc {      // written by the producer thread, read by everyone afte
     int e0, e1;         // non-zero range
     int halo;           // the block gathers columns owned by other ranks
     int q0, q1;         // windowed operators: the block's runs
-    int pad_;
+    int cb;             // narrow columns: the block's smallest column
 };
 static_assert(sizeof(BlockDesc) * kMaxStages <= 384 - 128, "descriptors overflow the header");
 
@@ -233,15 +252,18 @@ __device__ __forceinline__ BlockDesc load_desc(const CsrArgsT<P> &a, int b) {
     d.halo = q.x < 0;
     d.r0 = q.x < 0 ? ~q.x : q.x;
     d.r1 = q.y; d.e0 = q.z; d.e1 = q.w;
-    d.q0 = d.q1 = 0; d.pad_ = 0;
+    d.q0 = d.q1 = 0; d.cb = 0;
     if (FMT == FMT_WINDOW) {
         const int2 w = __ldg(a.wblk + b);
         d.q0 = w.x; d.q1 = w.y;
     }
+    if (FMT == FMT_COL16 || FMT == FMT_COL24) d.cb = __ldg(a.cbase + b);
     return d;
 }
 
 // Returns true if the block was staged (false: too long, use the strided path).
+// Every slice is its own bulk copy, its source aligned down to 16 bytes (the kernel adds back the
+// offset); the row pointers are the block-relative 16-bit ones of rows [r0, r1].
 template <int FMT = FMT_PLAIN, class P>
 __device__ __forceinline__ bool issue_block(const CsrArgsT<P> &a, const BlockDesc &d, char *stage,
                                             const StageLayout &lay, uint64_t *bar,
@@ -249,67 +271,55 @@ __device__ __forceinline__ bool issue_block(const CsrArgsT<P> &a, const BlockDes
     typedef typename P::TV TV;
     constexpr int VA = 16 / (int)sizeof(TV);        // values per 16 bytes
     const int nnz = d.e1 - d.e0;
-    if (FMT == FMT_PATTERN) {
-        // (a pattern-indexed operator has no long blocks)
-        const int a0 = d.e0 & ~(VA - 1);
-        const int nval = ((d.e1 - a0) + VA - 1) & ~(VA - 1);
-        const int nptr = ((d.r1 - d.r0 + 1) + 3) & ~3;
-        const int p0 = d.r0 & ~15;                  // pattern ids: 16 per 16 bytes
-        const int npid = ((d.r1 - p0) + 15) & ~15;
-        const uint32_t bytes = nval * (int)sizeof(TV) + nptr * 4 + npid;
-        ptx::mbar_expect_tx(bar, bytes);
-        if (nval) ptx::bulk_g2s(stage + lay.val_off, a.val + a0, nval * (int)sizeof(TV), bar, policy);
-        ptx::bulk_g2s(stage + lay.ptr_off, a.ptr + d.r0, nptr * 4, bar, policy);
-        ptx::bulk_g2s(stage + lay.pid_off, a.pid + p0, npid, bar, policy);
-        return true;
-    }
-    if (FMT == FMT_OFFSET) {
-        // (an offset-indexed operator has no long blocks)
-        const int a0 = d.e0 & ~(VA - 1);
-        const int nval = ((d.e1 - a0) + VA - 1) & ~(VA - 1);
-        const int c0 = d.e0 & ~15;                  // 8-bit columns: 16 per 16 bytes
-        const int ncol = ((d.e1 - c0) + 15) & ~15;
-        const int nptr = ((d.r1 - d.r0 + 1) + 3) & ~3;
-        const uint32_t bytes = nval * (int)sizeof(TV) + ncol + nptr * 4;
-        ptx::mbar_expect_tx(bar, bytes);
-        if (nval) ptx::bulk_g2s(stage + lay.val_off, a.val + a0, nval * (int)sizeof(TV), bar, policy);
-        if (ncol) ptx::bulk_g2s(stage + lay.col_off, a.idx8 + c0, ncol, bar, policy);
-        ptx::bulk_g2s(stage + lay.ptr_off, a.ptr + d.r0, nptr * 4, bar, policy);
-        return true;
-    }
-    if (FMT == FMT_WINDOW) {
-        // (a windowed operator has no long blocks)
-        const int a0 = d.e0 & ~(VA - 1);
-        const int nval = ((d.e1 - a0) + VA - 1) & ~(VA - 1);
-        const int c0 = d.e0 & ~7;                   // 16-bit columns: 8 per 16 bytes
-        const int ncol = ((d.e1 - c0) + 7) & ~7;
-        const int nptr = ((d.r1 - d.r0 + 1) + 3) & ~3;
-        const int qa = d.q0 & ~1;                   // runs: 2 per 16 bytes
-        const int nrun = ((d.q1 - qa) + 1) & ~1;
-        const uint32_t bytes = nval * (int)sizeof(TV) + ncol * 2 + nptr * 4 + nrun * 8;
-        ptx::mbar_expect_tx(bar, bytes);
-        if (nval) ptx::bulk_g2s(stage + lay.val_off, a.val + a0, nval * (int)sizeof(TV), bar, policy);
-        if (ncol) ptx::bulk_g2s(stage + lay.col_off, a.col16 + c0, ncol * 2, bar, policy);
-        ptx::bulk_g2s(stage + lay.ptr_off, a.ptr + d.r0, nptr * 4, bar, policy);
-        if (nrun) ptx::bulk_g2s(stage + lay.run_off, a.wrun + qa, nrun * 8, bar, policy);
-        return true;
-    }
-    if (nnz > a.nnz_cap) {
+    if (FMT == FMT_PLAIN && nnz > a.nnz_cap) {
         // nothing to stage: complete the phase with a plain arrive
+        // (only a plain operator has long blocks)
         asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(ptx::smem_addr(bar))
                      : "memory");
         return false;
     }
-    const int a0 = d.e0 & ~(VA - 1);                // val source aligned to 16 B
+    const int a0 = d.e0 & ~(VA - 1);
     const int nval = ((d.e1 - a0) + VA - 1) & ~(VA - 1);
-    const int c0 = d.e0 & ~3;                       // col source aligned to 16 B
-    const int ncol = ((d.e1 - c0) + 3) & ~3;
-    const int nptr = ((d.r1 - d.r0 + 1) + 3) & ~3;  // r0 is a multiple of 4
-    const uint32_t bytes = nval * (int)sizeof(TV) + ncol * 4 + nptr * 4;
+    const int p0 = d.r0 & ~7;                       // 16-bit row pointers: 8 per 16 bytes
+    const int nptr = ((d.r1 + 1 - p0) + 7) & ~7;  // (+ the next block's first row: 0)
+    int ncol = 0, nhi = 0, nrun = 0, npid = 0;      // bytes of each slice
+    const void *csrc = nullptr, *hsrc = nullptr, *psrc = nullptr;
+    if (FMT == FMT_PLAIN) {
+        const int c0 = d.e0 & ~3;
+        ncol = (((d.e1 - c0) + 3) & ~3) * 4;
+        csrc = a.col + c0;
+    } else if (FMT == FMT_WINDOW || FMT == FMT_COL16 || FMT == FMT_COL24) {
+        const int c0 = d.e0 & ~7;
+        ncol = (((d.e1 - c0) + 7) & ~7) * 2;
+        csrc = (FMT == FMT_WINDOW ? a.col16 : a.clo16) + c0;
+    } else if (FMT == FMT_OFFSET) {
+        const int c0 = d.e0 & ~15;
+        ncol = ((d.e1 - c0) + 15) & ~15;
+        csrc = a.idx8 + c0;
+    }
+    if (FMT == FMT_COL24) {
+        const int h0 = d.e0 & ~15;
+        nhi = ((d.e1 - h0) + 15) & ~15;
+        hsrc = a.chi8 + h0;
+    }
+    if (FMT == FMT_WINDOW) {
+        const int qa = d.q0 & ~1;                   // runs: 2 per 16 bytes
+        nrun = (((d.q1 - qa) + 1) & ~1) * 8;
+        psrc = a.wrun + qa;
+    }
+    if (FMT == FMT_PATTERN) {
+        const int q0 = d.r0 & ~15;                  // pattern ids: 16 per 16 bytes
+        npid = ((d.r1 - q0) + 15) & ~15;
+        psrc = a.pid + q0;
+    }
+    const uint32_t bytes = nval * (int)sizeof(TV) + ncol + nhi + nptr * 2 + nrun + npid;
     ptx::mbar_expect_tx(bar, bytes);
     if (nval) ptx::bulk_g2s(stage + lay.val_off, a.val + a0, nval * (int)sizeof(TV), bar, policy);
-    if (ncol) ptx::bulk_g2s(stage + lay.col_off, a.col + c0, ncol * 4, bar, policy);
-    ptx::bulk_g2s(stage + lay.ptr_off, a.ptr + d.r0, nptr * 4, bar, policy);
+    if (ncol) ptx::bulk_g2s(stage + lay.col_off, csrc, ncol, bar, policy);
+    if (nhi) ptx::bulk_g2s(stage + lay.hi_off, hsrc, nhi, bar, policy);
+    ptx::bulk_g2s(stage + lay.ptr_off, a.ptr16 + p0, nptr * 2, bar, policy);
+    if (nrun) ptx::bulk_g2s(stage + lay.run_off, psrc, nrun, bar, policy);
+    if (npid) ptx::bulk_g2s(stage + lay.pid_off, psrc, npid, bar, policy);
     return true;
 }
 
@@ -468,7 +478,8 @@ __device__ __forceinline__ void fill_window(const CsrArgsT<P> &a, const BlockDes
 // ---- reduce the rows of a staged block out of shared memory ---------------------
 // FMT_WINDOW: x comes from the block's window, `win`, indexed by the 16-bit columns;
 // FMT_OFFSET: the column of an entry of row r is r + off[8-bit index];
-// FMT_PATTERN: the column of the k-th entry of row r is r + off[pstart[pattern id of r] + k]
+// FMT_PATTERN: the column of the k-th entry of row r is r + off[pstart[pattern id of r] + k];
+// FMT_COL16 / FMT_COL24: the column is the block's smallest column + the stored 16 (+ 8) bits
 template <int MODE, int L, bool HALO, class P, int FMT = FMT_PLAIN>
 __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const BlockDesc &d,
                                                const char *stage, const StageLayout &lay, RowAcc &acc,
@@ -477,23 +488,36 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
     constexpr bool WIN = FMT == FMT_WINDOW;
     constexpr bool OFF = FMT == FMT_OFFSET;
     constexpr bool PAT = FMT == FMT_PATTERN;
+    constexpr bool NAR = FMT == FMT_COL16 || FMT == FMT_COL24;
     typedef typename P::TV TV;
     typedef typename P::TX TX;
     typedef typename P::TY TS;                       // row sums live in the output's type
-    typedef typename std::conditional<WIN, unsigned short,
+    typedef typename std::conditional<WIN || NAR, unsigned short,
                                       typename std::conditional<OFF, unsigned char, int>::type>::type CI;
-    static_assert(!((WIN || OFF || PAT) && L >= 16), "compressed column formats use at most 8 lanes per row");
+    static_assert(!((WIN || OFF || PAT || NAR) && L >= 16), "compressed column formats use at most 8 lanes per row");
     const unsigned char *pid_s = reinterpret_cast<const unsigned char *>(stage + lay.pid_off) + (d.r0 & 15);
     constexpr int VA = 16 / (int)sizeof(TV);
     const TV *val_s = reinterpret_cast<const TV *>(stage + lay.val_off);
     const CI     *col_s = reinterpret_cast<const CI *>(stage + lay.col_off);
-    const int    *ptr_s = reinterpret_cast<const int *>(stage + lay.ptr_off);
+    const unsigned char  *hi_s  = reinterpret_cast<const unsigned char *>(stage + lay.hi_off);
+    const unsigned short *ptr_s = reinterpret_cast<const unsigned short *>(stage + lay.ptr_off) + (d.r0 & 7);
     const int vo = d.e0 & ~(VA - 1);
-    const int co = WIN ? (d.e0 & ~7) : OFF ? (d.e0 & ~15) : (d.e0 & ~3);
+    const int nr = d.r1 - d.r0;
+    const int co = WIN || NAR ? (d.e0 & ~7) : OFF ? (d.e0 & ~15) : (d.e0 & ~3);
+    const int ho = d.e0 & ~15;
+    // what the stage holds for entry e: the column (plain, narrow) or its index (window, offset)
+    auto stored_col = [&](int e) -> int {
+        if (!NAR) return col_s[e - co];
+        if (FMT == FMT_COL24) return d.cb + ((int)col_s[e - co] | (int)hi_s[e - ho] << 16);
+        return d.cb + (int)col_s[e - co];
+    };
+    // row rr's entries, from the block-relative row pointers; the slot after the last row is
+    // the next block's first row, always 0: the last row ends at e1 = e0 + 0 + (e1 - e0)
+    auto row_beg = [&](int rr) -> int { return d.e0 + (int)ptr_s[rr]; };
+    auto row_end = [&](int rr) -> int { return d.e0 + (int)ptr_s[rr + 1] + (rr + 1 == nr ? d.e1 - d.e0 : 0); };
     constexpr int G = kThreads / L;
     const int g    = threadIdx.x / L;
     const int lane = threadIdx.x % L;
-    const int nr   = d.r1 - d.r0;
     const TX *__restrict__ x = a.x;
 
     if (L >= 16) {
@@ -512,8 +536,8 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
             for (int u = 0; u < RU; ++u) {
                 const int rr = base + u * G + g;
                 rowok[u] = rr < nr;
-                beg[u] = rowok[u] ? ptr_s[rr] : 0;
-                end[u] = rowok[u] ? ptr_s[rr + 1] : 0;
+                beg[u] = rowok[u] ? row_beg(rr) : 0;
+                end[u] = rowok[u] ? row_end(rr) : 0;
                 sum[u] = 0;
             }
             // first L entries of each of the RU rows: all loads first, then the gathers
@@ -521,7 +545,7 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
             for (int u = 0; u < RU; ++u) {
                 const int e = beg[u] + lane;
                 p[u] = e < end[u];
-                c[u] = p[u] ? col_s[e - co] : 0;
+                c[u] = p[u] ? stored_col(e) : 0;
                 v[u] = p[u] ? val_s[e - vo] : (TV)0;
             }
 #pragma unroll
@@ -533,7 +557,7 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
 #pragma unroll
             for (int u = 0; u < RU; ++u)
                 for (int e = beg[u] + lane + L; e < end[u]; e += L)
-                    sum[u] = fma((TS)val_s[e - vo], (TS)gather_m<MODE, HALO>(a, x, col_s[e - co]), sum[u]);
+                    sum[u] = fma((TS)val_s[e - vo], (TS)gather_m<MODE, HALO>(a, x, stored_col(e)), sum[u]);
 #pragma unroll
             for (int o = L / 2; o > 0; o >>= 1) {
 #pragma unroll
@@ -553,8 +577,8 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
         if (valid) {
             // the epilogue's operands travel with the row's gathers
             if (lane == 0) ops = load_row_ops<MODE>(a, d.r0 + rr);
-            const int beg = ptr_s[rr];
-            const int end = ptr_s[rr + 1];
+            const int beg = row_beg(rr);
+            const int end = row_end(rr);
             // PAT: the row's pattern starts at off[pb + beg], so entry e sits at off[pb + e]
             int pb = 0;
             if (PAT) pb = (int)pstart[pid_s[rr]] - beg;
@@ -570,7 +594,7 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
                     const int eu = e + u * L;
                     p[u] = eu < end;
                     if (PAT) c[u] = d.r0 + rr + off[pb + (p[u] ? eu : e)];
-                    else c[u] = p[u] ? col_s[eu - co] : col_s[e - co];
+                    else c[u] = stored_col(p[u] ? eu : e);
                 }
                 if (OFF) {
 #pragma unroll
@@ -700,7 +724,7 @@ __global__ void __launch_bounds__(kThreads, 4) csr_block_kernel(const CsrArgsT<P
 }
 
 // ---- variant 1: persistent CTAs, S-deep ring of stages ----------------------------------
-// FMT: storage format of the columns (FMT_PLAIN / FMT_WINDOW / FMT_OFFSET, see the top of the file)
+// FMT: storage format of the columns (FMT_*, see the top of the file)
 template <int MODE, int L, bool HALO, class P, int FMT = FMT_PLAIN>
 __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P> a, const int nstages) {
     extern __shared__ __align__(128) char smem[];
@@ -768,8 +792,9 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
                                                                             pstart_s);
         } else {
             if (!HALO) warm_lines(a, first + i * step);
+            // (plain or narrow columns; only a plain operator has long blocks)
             if ((d.e1 - d.e0) <= a.nnz_cap)
-                compute_staged<MODE, L, HALO>(a, d, stage, lay, acc);
+                compute_staged<MODE, L, HALO, P, FMT>(a, d, stage, lay, acc);
             else
                 compute_long<MODE, HALO>(a, d, red_s, acc);
         }

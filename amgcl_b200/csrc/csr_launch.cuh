@@ -1,6 +1,7 @@
 // csr_launch.cuh -- launching the persistent ring kernel (csr_kernels.cuh).  Shared by
 // api_matrices.cu (plain operators), api_window.cu (windowed operators), api_offsets.cu
-// (offset-indexed operators) and api_patterns.cu (pattern-indexed operators): the kernel instantiations of each storage format are compiled in
+// (offset-indexed operators), api_patterns.cu (pattern-indexed operators) and api_col16.cu /
+// api_col24.cu (narrow columns): the kernel instantiations of each storage format are compiled in
 // a translation unit of their own so the build stays parallel.
 #pragma once
 #include "internal.cuh"
@@ -60,6 +61,20 @@ int launch_ring_off(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
 // pattern-indexed operators (defined and instantiated in api_patterns.cu: 1..4 lanes per row)
 template <int MODE, int L, bool HALO, class P>
 int launch_ring_pat(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
+// narrow columns (api_col16.cu / api_col24.cu: 1..8 lanes per row)
+template <int MODE, int L, bool HALO, class P>
+int launch_ring_c16(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
+template <int MODE, int L, bool HALO, class P>
+int launch_ring_c24(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
+
+// the column format an operator is stored in (FMT_*)
+inline int stored_format(b200_csr_t A) {
+    if (A->pid) return FMT_PATTERN;
+    if (A->idx8) return FMT_OFFSET;
+    if (A->col16) return FMT_WINDOW;
+    if (A->narrow) return A->narrow == 24 ? FMT_COL24 : FMT_COL16;
+    return FMT_PLAIN;
+}
 
 // which storage format does this launch stream?
 template <class P>
@@ -71,6 +86,7 @@ inline int launch_format(b200_ctx_t ctx, b200_csr_t A) {
         int stages;
         if (ring_smem<P>(ctx, A, FMT_WINDOW, &stages) != 0) return FMT_WINDOW;
     }
+    if (A->narrow && ctx->opt_narrow && A->lanes <= 8) return A->narrow == 24 ? FMT_COL24 : FMT_COL16;
     return FMT_PLAIN;
 }
 

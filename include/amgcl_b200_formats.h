@@ -1,0 +1,57 @@
+/* amgcl_b200_formats.h -- the column formats of the CSR operators: which one each operator and
+ * each profiled pass uses, and the host-side plan of the narrow format.
+ *
+ * Kept apart from amgcl_b200.h on purpose: the drop-in library and the tutorial program are
+ * compiled from amgcl_b200.h together with AMGCL's headers, and a machine without AMGCL's
+ * headers can only install a kept build of them whose recorded source hash still matches.
+ * Nothing here is used by the AMGCL backend itself. */
+#ifndef AMGCL_B200_FORMATS_H
+#define AMGCL_B200_FORMATS_H
+
+#include "amgcl_b200.h"
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+/* Column formats, as b200_ctx_largest_operator and b200_profile_end_formats report them. */
+#define B200_FMT_PLAIN    0   /* int32 column per entry                                     */
+#define B200_FMT_WINDOW   1   /* 16-bit slot in a per-block shared-memory window of x       */
+#define B200_FMT_OFFSET   2   /* 8-bit index of col - row                                   */
+#define B200_FMT_PATTERN  3   /* no per-entry column: 8-bit row pattern id                  */
+#define B200_FMT_COL16    4   /* 16-bit column relative to the block's smallest column      */
+#define B200_FMT_COL24    5   /* the same in 24 bits (a 16-bit and an 8-bit array)          */
+
+/* Narrow columns.  Inside one row block the columns of an operator span far less than the
+ * int32 range.  An operator that is neither pattern- nor offset-indexed (nor windowed), has no
+ * long row blocks and at most 8 lanes per row stores, per row block, its smallest column and,
+ * per entry, the low 16 bits of (column - that base) plus, if some block spans more than
+ * 2^16 - 1 columns, the high 8 bits in a second array; the streaming kernel reads 2 or 3
+ * instead of 4 bytes of column per entry.  Same entry order and arithmetic, same bits.
+ * Context option "narrow_columns" (b200_ctx_set_option; env B200_NARROW_COLUMNS): 1 = built at
+ * upload and used (default), 0 = not built / not used.
+ * Every staged format streams 16-bit row pointers relative to the first non-zero of the row's
+ * block.
+ * b200_csr_narrow: 16 or 24, or 0 when A is not stored that way.
+ * b200_narrow_plan_i64: pure host helper for tests, the plan b200_csr_create builds for a
+ * single-GPU operator (base_out [nblocks], lo16_out / hi8_out [nnz], ptr16_out [nrows];
+ * width_out 0: stays plain). */
+int b200_csr_narrow(b200_csr_t A, int *width);
+int b200_narrow_plan_i64(int64_t nrows, int64_t ncols, const int64_t *ptr, const int64_t *col, int lanes,
+                         int nnz_cap, int32_t *base_out, int64_t base_capacity, uint16_t *lo16_out,
+                         uint8_t *hi8_out, uint16_t *ptr16_out, int64_t *nblocks_out, int *width_out);
+
+/* b200_profile_end with the column format each CSR pass streamed (B200_FMT_*; 0 for the other
+ * kernels).  Entries are aggregated per (shape, mode, format). */
+typedef struct {
+    b200_profile_entry entry;
+    int                format;
+} b200_profile_format_entry;
+int b200_profile_end_formats(b200_ctx_t ctx, b200_profile_format_entry *out, int64_t capacity,
+                             int64_t *count);
+
+#ifdef __cplusplus
+}
+#endif
+
+#endif /* AMGCL_B200_FORMATS_H */
