@@ -86,7 +86,6 @@ extern "C" int b200_ctx_create(int device, b200_ctx_t *out) {
     if (const char *e = getenv("B200_COARSE_TAIL")) ctx->opt_coarse_tail = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_FUSE_FIRST_SWEEP")) ctx->opt_fuse_first_sweep = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_POLL_SCALARS")) ctx->opt_poll_scalars = atoi(e) ? 1 : 0;
-    if (const char *e = getenv("B200_WARM_LINES")) ctx->opt_warm_lines = atoi(e);
     if (const char *e = getenv("B200_PATTERNS")) ctx->opt_patterns = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_PATTERNS_MIN_NNZ")) ctx->opt_patterns_min_nnz = atoll(e);
     if (const char *e = getenv("B200_OFFSETS")) ctx->opt_offsets = atoi(e) ? 1 : 0;
@@ -302,7 +301,6 @@ static int64_t *option_slot(b200_ctx_t ctx, const char *key) {
     if (!strcmp(key, "coarse_tail")) return &ctx->opt_coarse_tail;
     if (!strcmp(key, "poll_scalars")) return &ctx->opt_poll_scalars;
     if (!strcmp(key, "small_kernel_max_nnz")) return &ctx->opt_small_kernel_max_nnz;
-    if (!strcmp(key, "warm_lines")) return &ctx->opt_warm_lines;
     if (!strcmp(key, "patterns")) return &ctx->opt_patterns;
     if (!strcmp(key, "patterns_min_nnz")) return &ctx->opt_patterns_min_nnz;
     if (!strcmp(key, "offsets")) return &ctx->opt_offsets;

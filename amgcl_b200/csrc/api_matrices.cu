@@ -233,6 +233,17 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     A->dtype = std::is_same<Val, float>::value ? B200_F32 : B200_F64;
     A->lanes = lanes; A->rows_cap = rows_cap; A->nnz_cap = nnz_cap;
     A->nblocks = nblocks; A->nlong = nlong;
+    {
+        // blocks with fewer chunks of 32 / lanes rows than the CTA has warps (csr_ring_kernel)
+        const int rw = 32 / lanes;
+        int64_t few = 0;
+        for (int64_t b = 0; b < nblocks; ++b) {
+            const int4 q = blk4[(size_t)b];
+            const int nr = q.y - (q.x < 0 ? ~q.x : q.x);
+            if (q.w - q.z <= nnz_cap && (nr + rw - 1) / rw < kThreads / 32) ++few;
+        }
+        A->row_stream = 2 * few > nblocks;
+    }
     // padding: bulk copies round sizes up to 16 bytes
     const size_t ptr_bytes = ((size_t)nrows + 1 + 8) * sizeof(int);
     const size_t col_bytes = ((size_t)nnz + 8) * sizeof(int);
@@ -348,44 +359,6 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
         ctx->big_fmt = stored_format(A);
     }
     *out = A;
-    if (halo_from < 0 && !windowed && ctx->opt_warm_lines && lanes >= 2 && A->dtype == B200_F64 && nblocks > 0 &&
-        (ctx->opt_warm_lines > 1 || nnz >= 1000000)) {
-        // Gather-heavy operator: the 128-byte lines of x every row block gathers from (sorted,
-        // distinct), so the kernel can fill them into L1 with a few coalesced loads instead of
-        // one sector miss per scattered gather (warm_lines, csr_kernels.cuh).
-        std::vector<std::vector<int>> per((size_t)nblocks);
-#pragma omp parallel for schedule(dynamic, 64)
-        for (int64_t b = 0; b < nblocks; ++b) {
-            const int64_t e0 = blk[(size_t)b].y, e1 = blk[(size_t)b + 1].y;
-            std::vector<int> &v = per[(size_t)b];
-            v.reserve((size_t)(e1 - e0));
-            for (int64_t e = e0; e < e1; ++e) v.push_back((int)((int64_t)col[e] >> 4));
-            std::sort(v.begin(), v.end());
-            v.erase(std::unique(v.begin(), v.end()), v.end());
-            if (v.size() > 192) v.clear();              // too scattered to be worth touching
-        }
-        std::vector<int> wptr((size_t)nblocks + 1, 0);
-        for (int64_t b = 0; b < nblocks; ++b) wptr[(size_t)b + 1] = wptr[(size_t)b] + (int)per[(size_t)b].size();
-        std::vector<int> wl((size_t)wptr[(size_t)nblocks]);
-#pragma omp parallel for schedule(static)
-        for (int64_t b = 0; b < nblocks; ++b)
-            std::copy(per[(size_t)b].begin(), per[(size_t)b].end(), wl.begin() + wptr[(size_t)b]);
-        cudaError_t rc = cudaMalloc(&A->wl_ptr, wptr.size() * sizeof(int));
-        if (rc == cudaSuccess) rc = cudaMalloc(&A->wl, std::max<size_t>(1, wl.size()) * sizeof(int));
-        if (rc == cudaSuccess) rc = cudaMemcpyAsync(A->wl_ptr, wptr.data(), wptr.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream);
-        if (rc == cudaSuccess && !wl.empty())
-            rc = cudaMemcpyAsync(A->wl, wl.data(), wl.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream);
-        if (rc == cudaSuccess) rc = cudaStreamSynchronize(ctx->stream);
-        if (rc != cudaSuccess) {
-            cudaGetLastError();                         // an optimisation only: run without it
-            if (A->wl_ptr) cudaFree(A->wl_ptr);
-            if (A->wl) cudaFree(A->wl);
-            A->wl_ptr = A->wl = nullptr;
-        } else {
-            A->wl_count = (int64_t)wl.size();
-            A->bytes += (wptr.size() + wl.size()) * sizeof(int);
-        }
-    }
     return B200_OK;
 }
 
@@ -395,8 +368,6 @@ static void csr_free(b200_csr_t A) {
     if (A->col) cudaFree(A->col);
     if (A->val) cudaFree(A->val);
     if (A->blk) cudaFree(A->blk);
-    if (A->wl_ptr) cudaFree(A->wl_ptr);
-    if (A->wl) cudaFree(A->wl);
     if (A->col16) cudaFree(A->col16);
     if (A->wrun) cudaFree(A->wrun);
     if (A->wblk) cudaFree(A->wblk);
@@ -614,8 +585,7 @@ static CsrArgsT<P> base_args_t(b200_csr_t A) {
     memset(&a, 0, sizeof(a));
     a.ptr = A->ptr; a.ptr16 = A->ptr16; a.col = A->col; a.val = static_cast<const typename P::TV *>(A->val); a.blk = A->blk;
     a.nrows = (int)A->nrows; a.nblocks = (int)A->nblocks;
-    a.rows_cap = A->rows_cap; a.nnz_cap = A->nnz_cap;
-    if (std::is_same<P, PrecDD>::value && A->ctx->opt_warm_lines) { a.wl_ptr = A->wl_ptr; a.wl = A->wl; }
+    a.rows_cap = A->rows_cap; a.nnz_cap = A->nnz_cap; a.row_stream = A->row_stream;
     a.col16 = A->col16; a.wrun = A->wrun; a.wblk = A->wblk; a.run_cap = A->win_runs;
     a.idx8 = A->idx8; a.off_tab = A->off_tab;
     a.pid = A->pid; a.pat_start = A->pat_start; a.pat_off = A->pat_off; a.pat_total = A->pat_total;

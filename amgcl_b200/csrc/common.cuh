@@ -170,8 +170,6 @@ struct b200_ctx_s {
     int64_t opt_window_ratio  = 75;       // ... windows no larger than this percentage of the entries,
     int64_t opt_window_gap    = 2;        // ... runs are merged across holes of (gap - 1) sectors
     int64_t opt_window_lanes  = 15;       // ... lanes per row in this set (bit k: 2^k lanes)
-    int64_t opt_warm_lines    = 0;        // gather-heavy operators: touch a block's lines of x before reducing it
-                                          // (opt-in experiment: measured no gain, DESIGN.md section 8)
     int64_t opt_small_kernel_max_nnz = 0;         // FP64 operators up to this size: direct-load kernel
                                                   // (opt-in: measured slower than the ring kernel, DESIGN.md)
     int64_t opt_fused_krylov  = 1;        // the C++ binding's cg / bicgstab use the fused b200_cg_* / b200_bicg_* steps
@@ -260,9 +258,8 @@ struct b200_csr_s {
     int        nnz_cap  = 2048;   // staged non-zeros per block
     int64_t    nblocks  = 0;
     int64_t    nlong    = 0;      // blocks too long to stage (handled by the strided path)
-    int       *wl_ptr   = nullptr;// gather-heavy operators: [nblocks+1] offsets into wl (walk order)
-    int       *wl       = nullptr;// 128-byte lines of x each row block gathers from
-    int64_t    wl_count = 0;
+    bool       row_stream = false;// most blocks leave warps without rows: no CTA barrier between
+                                  //   blocks (csr_ring_kernel)
     // windowed operators (csr_kernels.cuh): blocks gather x from a shared-memory window
     unsigned short *col16 = nullptr;  // [nnz] (+ padding) window-local column of every entry
     int2      *wrun     = nullptr;// runs of x the windows are made of {first column, len | slot << 16}

@@ -59,8 +59,9 @@
 // the high 8 bits in an array of their own where some block spans more than 16 bits
 // (narrow.cuh): 2 or 3 instead of 4 bytes of column per entry.
 //
-// Between blocks the CTA synchronises with a barrier (plain, windowed) or not at all
-// (offset- / pattern-indexed: the last warp done with a stage refills it) -- see the ring kernel.
+// The rows of the blocks a CTA walks form one stream over its warps.  Between blocks the CTA
+// synchronises with a barrier (windowed; plain and narrow operators whose blocks give every warp
+// rows) or not at all (the last warp done with a stage refills it) -- see the ring kernel.
 //
 // Precision.  Every kernel is a template over the element types of the matrix
 // values, the gathered vector, the right-hand side, the output and the smoother
@@ -124,6 +125,7 @@ struct CsrArgsT {
     int           nblocks;
     int           rows_cap;
     int           nnz_cap;
+    int           row_stream;     // plain / narrow formats: no CTA barrier between blocks (ring kernel)
     const typename P::TX *x;      // gathered vector (local columns)
     const typename P::TX *xh;     // halo values for columns >= nloc (multi-GPU), else nullptr
     int           nloc;   // number of local columns when xh is set
@@ -152,12 +154,6 @@ struct CsrArgsT {
     unsigned long long       *gather_flag[kMaxRanks];
     unsigned int             *gather_ticket;
     unsigned long long        gather_seq;
-    // Gather-heavy operators (long rows): the 128-byte lines of x a row block gathers from, as a
-    // per-block list (built at upload).  Before reducing a block the CTA touches each of them
-    // once with coalesced loads -- one L2->L1 fill per LINE the block uses, instead of one
-    // 32-byte sector fill per scattered 8-byte gather that misses (warm_lines below).
-    const int    *wl_ptr; // [nblocks+1] (walk order) or nullptr
-    const int    *wl;     // line numbers (x index / 16)
     // Windowed operators: window-local column of every entry, the runs of x each block's window
     // is made of ({first column, length | first slot << 16}), and each block's range of runs
     const unsigned short *col16;
@@ -437,22 +433,6 @@ __device__ __forceinline__ void wait_for_halo(const CsrArgsT<P> &a, const BlockD
     __syncthreads();
 }
 
-// ---- bring the lines of x a block gathers from into L1 with coalesced loads --------------
-// Four threads per 128-byte line, one 8-byte load per 32-byte sector; the values are not used.
-// The gathers that follow hit (or merge with the outstanding fills).
-template <class P>
-__device__ __forceinline__ void warm_lines(const CsrArgsT<P> &a, int pos) {
-    if (a.wl_ptr == nullptr) return;
-    const int w0 = __ldg(a.wl_ptr + pos), w1 = __ldg(a.wl_ptr + pos + 1);
-    const char *base = reinterpret_cast<const char *>(a.x);
-    for (int t = w0 * 4 + (int)threadIdx.x; t < w1 * 4; t += kThreads) {
-        const int line = __ldg(a.wl + (t >> 2));
-        const char *p = base + (size_t)line * 128 + (size_t)(t & 3) * 32;
-        unsigned long long sink;
-        asm volatile("ld.global.ca.u64 %0, [%1];" : "=l"(sink) : "l"(p) : "memory");
-    }
-}
-
 // ---- windowed operators: bring the block's runs of x into shared memory --------------------
 // One warp per run (runs are at most kWinRunLen long and start on a 32-byte boundary of x, so a
 // warp's loads are whole sectors); ends with a CTA barrier.
@@ -480,11 +460,15 @@ __device__ __forceinline__ void fill_window(const CsrArgsT<P> &a, const BlockDes
 // FMT_OFFSET: the column of an entry of row r is r + off[8-bit index];
 // FMT_PATTERN: the column of the k-th entry of row r is r + off[pstart[pattern id of r] + k];
 // FMT_COL16 / FMT_COL24: the column is the block's smallest column + the stored 16 (+ 8) bits
+//
+// Rows go to warps in chunks of 32 / L rows: chunk j of the block (rows [j*32/L, (j+1)*32/L)) is
+// reduced by warp (k0 + j) % 8, one row per group of L lanes.  k0 is the block's first chunk in
+// the CTA's stream of rows (csr_ring_kernel); with k0 = 0 warp w takes chunks w, w + 8, ...
 template <int MODE, int L, bool HALO, class P, int FMT = FMT_PLAIN>
 __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const BlockDesc &d,
                                                const char *stage, const StageLayout &lay, RowAcc &acc,
                                                const typename P::TX *win = nullptr, const int *off = nullptr,
-                                               const unsigned short *pstart = nullptr) {
+                                               const unsigned short *pstart = nullptr, int k0 = 0) {
     constexpr bool WIN = FMT == FMT_WINDOW;
     constexpr bool OFF = FMT == FMT_OFFSET;
     constexpr bool PAT = FMT == FMT_PATTERN;
@@ -516,7 +500,8 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
     auto row_beg = [&](int rr) -> int { return d.e0 + (int)ptr_s[rr]; };
     auto row_end = [&](int rr) -> int { return d.e0 + (int)ptr_s[rr + 1] + (rr + 1 == nr ? d.e1 - d.e0 : 0); };
     constexpr int G = kThreads / L;
-    const int g    = threadIdx.x / L;
+    const int c0   = (((int)threadIdx.x >> 5) - k0) & (kThreads / 32 - 1);   // this warp's first chunk
+    const int g    = (threadIdx.x & 31) / L;                                   // its row in a chunk
     const int lane = threadIdx.x % L;
     const TX *__restrict__ x = a.x;
 
@@ -526,7 +511,7 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
         // row coalesce.  Memory-level parallelism comes from working on RU rows at once
         // instead of batching along one (short) row.
         constexpr int RU = kGatherBatch;
-        for (int base = 0; base < nr; base += G * RU) {
+        for (int base = c0 * (32 / L); base < nr; base += G * RU) {
             int  beg[RU], end[RU], c[RU];
             TV   v[RU];
             TX   xv[RU];
@@ -568,7 +553,7 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
                 if (rowok[u] && lane == 0) store_row<MODE>(a, d.r0 + base + u * G + g, sum[u], acc);
         }
     } else
-    for (int base = 0; base < nr; base += G) {
+    for (int base = c0 * (32 / L); base < nr; base += G) {
         const int  rr    = base + g;
         const bool valid = rr < nr;
         TS sum = 0;
@@ -769,36 +754,41 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
     ptx::pdl_wait();         // vectors (x, f, d, y) come from earlier kernels: from here on
     if (HALO) halo_push(a);  // multi-GPU: my boundary values go out before anything else
 
+    // The rows of the blocks a CTA walks form one stream, cut into chunks of one warp's worth of
+    // rows (32 / L); chunk k of the stream goes to warp k % 8 (compute_staged), a fixed function of
+    // the blocks' row counts, so the in-kernel scalars stay deterministic.
+    // Decoupled: no CTA barrier between blocks.  A warp that is done with its chunks of a block
+    // moves on to the next stage at once, and the LAST warp to finish refills the stage.  Warps
+    // thus stay busy when a block has fewer rows than the CTA has row groups (long-row operators:
+    // about 68 rows per block for 128 groups at 2 lanes per row, DESIGN.md section 3.1b).
+    // Every warp waits on and arrives for every block, also one it has no chunk of: it reads the
+    // block's descriptor, and no warp may fall a whole phase of a stage's mbarrier behind.
+    // A long block (plain format) takes the whole CTA: the barriers of compute_long drain the
+    // stream up to it.  Offset- and pattern-indexed operators always run decoupled; plain and
+    // narrow ones where most blocks leave a warp without rows (a.row_stream, set at upload):
+    // where every warp has rows anyway (the prolongation of the finest level, 256 rows of about 4
+    // entries per block) the block-synchronous release measured faster.  The windowed format fills
+    // its window with the whole CTA: block-synchronous.
+    const bool decoupled = FMT == FMT_OFFSET || FMT == FMT_PATTERN || (FMT != FMT_WINDOW && a.row_stream);
+    constexpr int LS = FMT == FMT_PLAIN || L < 16 ? L : 8;   // (compressed formats: at most 8 lanes)
     RowAcc acc = {0.0, 0.0};
+    int k0 = 0;                    // the current block's first chunk in the CTA's stream of rows
     int s = 0, parity = 0;
     for (int i = 0; i < mine; ++i) {
         ptx::mbar_wait(bars + s, parity);
         const BlockDesc d = descs[s];
         wait_for_halo<HALO>(a, d);
         const char *stage = stages + (size_t)s * lay.bytes;
-        // Compressed formats (the short-row finest operator): no CTA barrier between blocks -- a
-        // warp that is done with this block moves on to the next stage at once, and the LAST
-        // warp to finish refills the stage.  Measured on the 256^3 solve: -5 % on those passes;
-        // on the plain-format operators (long rows, half of the warps without rows in a block)
-        // the same scheme costs 10-15 %, so they stay block-synchronous.
-        constexpr bool kDecoupled = FMT == FMT_OFFSET || FMT == FMT_PATTERN;
         if constexpr (FMT == FMT_WINDOW) {
             fill_window<MODE, HALO>(a, d, stage, lay, win);
-            compute_staged<MODE, (L < 16 ? L : 8), HALO, P, FMT_WINDOW>(a, d, stage, lay, acc, win);
-        } else if constexpr (FMT == FMT_OFFSET) {
-            compute_staged<MODE, (L < 16 ? L : 8), HALO, P, FMT_OFFSET>(a, d, stage, lay, acc, nullptr, off_s);
-        } else if constexpr (FMT == FMT_PATTERN) {
-            compute_staged<MODE, (L < 16 ? L : 8), HALO, P, FMT_PATTERN>(a, d, stage, lay, acc, nullptr, off_s,
-                                                                            pstart_s);
+            compute_staged<MODE, LS, HALO, P, FMT_WINDOW>(a, d, stage, lay, acc, win);
+        } else if (FMT != FMT_PLAIN || (d.e1 - d.e0) <= a.nnz_cap) {
+            compute_staged<MODE, LS, HALO, P, FMT>(a, d, stage, lay, acc, nullptr, off_s, pstart_s, k0);
+            k0 += (d.r1 - d.r0 + 32 / LS - 1) / (32 / LS);
         } else {
-            if (!HALO) warm_lines(a, first + i * step);
-            // (plain or narrow columns; only a plain operator has long blocks)
-            if ((d.e1 - d.e0) <= a.nnz_cap)
-                compute_staged<MODE, L, HALO, P, FMT>(a, d, stage, lay, acc);
-            else
-                compute_long<MODE, HALO>(a, d, red_s, acc);
+            compute_long<MODE, HALO>(a, d, red_s, acc);
         }
-        if constexpr (kDecoupled) {
+        if (decoupled) {
             // its arrive.expect_tx (release) / the others' wait (acquire) on the stage's mbarrier
             // publish the new descriptor; the counter orders everyone's reads of the stage before
             // the refill
