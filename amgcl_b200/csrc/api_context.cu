@@ -362,16 +362,18 @@ static void graph_free(b200_graph_s *g) {
     if (g->graph) cudaGraphDestroy(g->graph);
     delete g;
 }
-// put every touched object back into the state it had when recording started (nothing that
-// was recorded has run)
 static void graph_release_deferred(b200_ctx_t ctx) {
     for (void *p : ctx->graph_deferred) cudaFree(p);     // cudaFree waits for the device
     ctx->graph_deferred.clear();
 }
+// put every touched object back into the state it had when recording started (nothing that
+// was recorded has run).  The generations move on rather than back: products the recorded
+// calls registered name table slots no executed kernel wrote, and must not match.
 static void graph_rollback(b200_graph_s *g) {
     for (const GraphSlot &s : g->slots) {
         *s.slot = s.p0;
         if (s.zp) *s.zp = s.z0;
+        if (s.gen) ++*s.gen;
     }
 }
 } // namespace b200

@@ -300,7 +300,9 @@ extern "C" int b200_clear(b200_ctx_t ctx, b200_vec_t x) {
         if (ctx->lazy_vec == x) ctx->lazy_vec = nullptr;
     }
     x->gen++;
-    if (ctx->opt_zero_shortcut) {
+    // memory the caller can see (wrapped, or its raw pointer handed out) is cleared at once:
+    // the caller reads it behind the library's back
+    if (ctx->opt_zero_shortcut && x->owned && !x->escaped) {
         x->zero_pending = true;
         return B200_OK;
     }
@@ -315,10 +317,7 @@ extern "C" int b200_copy(b200_ctx_t ctx, b200_vec_t x, b200_vec_t y) {
     touch(ctx, {x, y});
     B200_REQUIRE(same_layout(x, y), "copy: size mismatch");
     if (x == y || x->ptr == y->ptr) return B200_OK;
-    if (x->zero_pending) {
-        y->zero_pending = true;
-        return B200_OK;
-    }
+    if (x->zero_pending) return b200_clear(ctx, y);     // drops a pending sweep of y, bumps its gen
     GUARD(ctx);
     if (all64({x, y}))
         return launch_ew<CopyF<double>, false, false, double>(ctx, x->len, CopyF<double>(), x->ptr, nullptr, nullptr, wr(y));
