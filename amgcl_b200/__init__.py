@@ -21,7 +21,7 @@ from . import build as _build
 
 __all__ = ["lib", "dropin_lib", "Context", "Vector", "Csr", "Coarse", "Krylov", "DropinSolver",
            "poisson3d", "unstructured3d", "B200Error", "RELAX", "KRYLOV", "nccl_unique_id",
-           "partition", "dist_split"]
+           "partition", "dist_split", "coarse_lu_plan"]
 
 _c = ctypes
 _i64 = _c.c_int64
@@ -55,7 +55,7 @@ FORMAT_NAMES = ("plain", "window", "offset", "pattern", "col16", "col24")
 # vecK: element-wise pass over K+1 vector streams (reads + writes)
 MODE_NAMES = {0: "spmv", 1: "spmv_acc", 2: "residual", 3: "relax", 4: "residual_scaled", 10: "vec1", 11: "vec2",
               12: "vec3", 13: "vec4", 14: "vec5", 15: "vec6", 16: "vec7",
-              20: "dot", 21: "relax_zero", 22: "coarse_gemv", 23: "memset", 24: "coarse_tail",
+              20: "dot", 21: "relax_zero", 22: "coarse_gemv", 23: "memset", 24: "coarse_tail", 25: "coarse_lu",
               30: "comm"}
 
 
@@ -130,6 +130,9 @@ def lib():
         "b200_coarse_create_i32": [_vp, _i64, _vp, _vp, _vp, _P(_vp)],
         "b200_coarse_destroy": [_vp],
         "b200_coarse_bytes": [_vp, _P(_c.c_size_t)],
+        "b200_coarse_info": [_vp, _P(_c.c_int), _P(_i64), _P(_i64), _P(_i64)],
+        "b200_coarse_lu_plan_i64": [_i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _P(_i64), _P(_c.c_int),
+                                    _P(_i64), _P(_c.c_size_t), _P(_c.c_size_t)],
         "b200_coarse_solve": [_vp, _vp, _vp, _vp],
         "b200_nccl_unique_id": [_c.c_char_p, _c.c_size_t],
         "b200_dist_init": [_vp, _c.c_char_p, _c.c_size_t, _c.c_int, _c.c_int, _i64],
@@ -665,8 +668,36 @@ def window_plan(nrows, ncols, ptr, col, lanes=0, nnz_cap=2048, slot_cap=1400, ma
             "max_runs": mr.value}
 
 
+def coarse_lu_plan(n, ptr, col):
+    """Symbolic phase of the banded-LU coarse solver for a host matrix (b200_coarse_lu_plan_i64,
+    no device needed): a dict with perm (perm[new] = old), lower / upper (per-row lower and
+    per-column upper bandwidth of the permuted matrix), lfirst / ulast (per tile, the first
+    and last tile its L and U panels reach), tile_rows, bandwidth, factor_bytes, setup_bytes."""
+    L = lib()
+    n = int(n)
+    ptr = np.ascontiguousarray(ptr, dtype=np.int64)
+    col = np.ascontiguousarray(col, dtype=np.int64)
+    tiles, rows, bw = _i64(), _c.c_int(), _i64()
+    fb, sb = _c.c_size_t(), _c.c_size_t()
+    _check(L.b200_coarse_lu_plan_i64(n, _ptr(ptr), _ptr(col), None, None, None, None, None, 0,
+                                     _c.byref(tiles), _c.byref(rows), _c.byref(bw), _c.byref(fb),
+                                     _c.byref(sb)), "b200_coarse_lu_plan_i64")
+    perm = np.empty(n, dtype=np.int32)
+    lower = np.empty(n, dtype=np.int32)
+    upper = np.empty(n, dtype=np.int32)
+    lfirst = np.empty(tiles.value, dtype=np.int64)
+    ulast = np.empty(tiles.value, dtype=np.int64)
+    _check(L.b200_coarse_lu_plan_i64(n, _ptr(ptr), _ptr(col), _ptr(perm), _ptr(lower), _ptr(upper),
+                                     _ptr(lfirst), _ptr(ulast), tiles.value, None, None, None, None, None),
+           "b200_coarse_lu_plan_i64")
+    return {"perm": perm, "lower": lower, "upper": upper, "lfirst": lfirst, "ulast": ulast,
+            "tile_rows": rows.value, "bandwidth": bw.value, "factor_bytes": fb.value,
+            "setup_bytes": sb.value}
+
+
 class Coarse:
-    """Coarsest-level device solver (b200_coarse_t)."""
+    """Coarsest-level device solver (b200_coarse_t): the dense inverse up to 16384 rows, a
+    banded LU above."""
 
     def __init__(self, ctx, n, ptr, col, val):
         self.ctx = ctx
@@ -677,6 +708,20 @@ class Coarse:
         _check(lib().b200_coarse_create_i64(ctx.h, int(n), _ptr(ptr), _ptr(col), _ptr(val),
                                             _c.byref(self.h)), "b200_coarse_create")
         self.n = int(n)
+
+    COARSE_KINDS = ("dense_inverse", "banded_lu")
+
+    def info(self):
+        """{kind: 'dense_inverse' | 'banded_lu', n, bandwidth, tiles} (b200_coarse_info)."""
+        k, n, bw, t = _c.c_int(), _i64(), _i64(), _i64()
+        _check(lib().b200_coarse_info(self.h, _c.byref(k), _c.byref(n), _c.byref(bw), _c.byref(t)),
+               "b200_coarse_info")
+        return {"kind": self.COARSE_KINDS[k.value], "n": n.value, "bandwidth": bw.value, "tiles": t.value}
+
+    def bytes(self):
+        b = _c.c_size_t()
+        _check(lib().b200_coarse_bytes(self.h, _c.byref(b)), "b200_coarse_bytes")
+        return b.value
 
     def __del__(self):
         try:

@@ -75,7 +75,8 @@ def build_cuda(force=False, verbose=False):
     os.makedirs(LIBDIR, exist_ok=True)
     units, headers = cuda_sources()
     deps = [os.path.join(CSRC, f) for f in headers] + [os.path.join(INCLUDE, "amgcl_b200.h"),
-                                                         os.path.join(INCLUDE, "amgcl_b200_formats.h")]
+                                                         os.path.join(INCLUDE, "amgcl_b200_formats.h"),
+                                                         os.path.join(INCLUDE, "amgcl_b200_coarse.h")]
     if not force and not _newer(LIB_CUDA, deps + [os.path.join(CSRC, u) for u in units]):
         return LIB_CUDA
     nvcc = nvcc_path()

@@ -1,4 +1,5 @@
-// api_coarse.cu -- coarsest-level direct solver (dense inverse on the device)
+// api_coarse.cu -- coarsest-level direct solver (dense inverse on the device; levels above
+// kCoarseDenseMax rows go to the banded LU of api_coarse_lu.cu)
 //
 // Part of the implementation of the C ABI declared in include/amgcl_b200.h (host-side logic
 // only: argument checking, bookkeeping, kernel launches; no CPU fallback anywhere).
@@ -19,7 +20,11 @@ static int coarse_create(b200_ctx_t ctx, int64_t n, const Ptr *ptr, const Col *c
     NOT_RECORDING(ctx, "coarse solver creation");
     B200_REQUIRE(out != nullptr, "null output pointer");
     *out = nullptr;
-    B200_REQUIRE(n > 0 && n <= 16384, "coarse solver: n must be in [1, 16384]");
+    B200_REQUIRE(n > 0, "coarse solver: n must be positive");
+    B200_REQUIRE(!ctx->dist || n <= kCoarseDenseMax,
+                 "coarse solver: a multi-GPU context solves coarsest levels of at most 16384 rows "
+                 "(lower coarse_enough)");
+    B200_REQUIRE(n < ((int64_t)1 << 31), "coarse solver: n does not fit int32");
     B200_REQUIRE(ptr && ptr[0] == 0, "bad row pointer array");
     const int64_t nnz = (int64_t)ptr[n];
     B200_REQUIRE(nnz >= 0 && (nnz == 0 || (col && val)), "bad col/val array");
@@ -40,6 +45,18 @@ static int coarse_create(b200_ctx_t ctx, int64_t n, const Ptr *ptr, const Col *c
     // the inverse is always formed and kept in FP64, whatever the hierarchy's precision
     std::vector<double> hval((size_t)nnz);
     for (int64_t e = 0; e < nnz; ++e) hval[(size_t)e] = (double)val[e];
+    if (n > kCoarseDenseMax) {
+        for (int64_t i = 0; i < n; ++i)
+            if (hptr[(size_t)i + 1] < hptr[(size_t)i]) return fail(B200_EINVAL, "bad row pointer array");
+        b200_coarse_s *S = new (std::nothrow) b200_coarse_s();
+        if (!S) return fail(B200_ENOMEM, "out of host memory");
+        S->ctx = ctx; S->n = n;
+        S->dtype = std::is_same<Val, float>::value ? B200_F32 : B200_F64;
+        const int rc = coarse_lu_create(ctx, n, hptr, hcol, hval, S);
+        if (rc) { delete S; return rc; }
+        *out = S;
+        return B200_OK;
+    }
     const int N = (int)n;
     int *dptr = nullptr, *dcol = nullptr, *dpiv = nullptr;
     double *dval = nullptr, *M = nullptr, *colk = nullptr, *pivval = nullptr, *Ainv = nullptr;
@@ -163,6 +180,7 @@ extern "C" int b200_coarse_destroy(b200_coarse_t S) {
     if (S->in_graph) S->ctx->destroy_epoch++;
     GUARD(S->ctx);
     if (S->Ainv) cudaFree(S->Ainv);
+    coarse_lu_destroy(S->lu);
     if (S->gbuf) cudaFree(S->gbuf);
     delete S;
     return B200_OK;
@@ -215,6 +233,7 @@ extern "C" int b200_coarse_solve(b200_ctx_t ctx, b200_coarse_t S, b200_vec_t rhs
                  "coarse solve: vectors must live on this rank");
     B200_REQUIRE(rhs != x && rhs->ptr != x->ptr, "coarse solve: rhs and x must not alias");
     if (rhs->dtype != x->dtype) return B200_BAD_MIX("coarse solve");
+    if (S->lu) return coarse_lu_solve(ctx, S, rhs, x);        // flushes the coarse tail
     const double *pr;
     int rc = rd(rhs, &pr);
     if (rc) return rc;

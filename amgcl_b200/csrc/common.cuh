@@ -13,6 +13,7 @@
 
 #include "../../include/amgcl_b200.h"
 #include "../../include/amgcl_b200_formats.h"
+#include "../../include/amgcl_b200_coarse.h"
 
 namespace b200 {
 
@@ -297,8 +298,12 @@ struct b200_index_s {
     bool       in_graph = false;
 };
 
+namespace b200 { struct CoarseLu; }   // banded LU factor (api_coarse_lu.cu)
+
 struct b200_coarse_s {
     b200_ctx_t ctx  = nullptr;
+    int        kind = B200_COARSE_DENSE;  // which representation was built (from n alone)
+    b200::CoarseLu *lu = nullptr;         // B200_COARSE_BANDED_LU: the factor and sweep state
     int        dtype = B200_F64;  // element type of the vectors it is applied to
     bool       replicated = false;// multi-GPU: coarsest level partitioned -> inverse on every rank
     double    *gbuf = nullptr;    // replicated: all-gathered right-hand side [nranks * block]

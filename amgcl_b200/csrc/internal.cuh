@@ -85,6 +85,14 @@ struct TailHold {
     ~TailHold() { ctx->tail_hold = prev; }
 };
 
+// ---- implemented in api_coarse_lu.cu: the coarsest level above the dense inverse's size -----
+constexpr int64_t kCoarseDenseMax = 16384;   // largest n the dense inverse takes
+int  coarse_lu_create(b200_ctx_t ctx, int64_t n, const std::vector<int32_t> &ptr,
+                      const std::vector<int32_t> &col, const std::vector<double> &val,
+                      b200_coarse_s *S);
+int  coarse_lu_solve(b200_ctx_t ctx, b200_coarse_s *S, b200_vec_t rhs, b200_vec_t x);
+void coarse_lu_destroy(CoarseLu *lu);
+
 // ---- implemented in api_matrices.cu: the lazy first smoother sweep ---------------------------
 int  lazy_flush(b200_ctx_t ctx);        // write out the pending x = (omega*d).*f, if any
 
