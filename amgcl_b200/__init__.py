@@ -45,7 +45,7 @@ class ProfileEntry(_c.Structure):
 
 class ProfileFormatEntry(_c.Structure):
     """b200_profile_format_entry (include/amgcl_b200_formats.h)."""
-    _fields_ = [("entry", ProfileEntry), ("format", _c.c_int)]
+    _fields_ = [("entry", ProfileEntry), ("format", _c.c_int), ("value_bytes", _c.c_int)]
 
 
 # column formats of a CSR operator (include/amgcl_b200_formats.h B200_FMT_*)
@@ -150,6 +150,8 @@ def lib():
         "b200_csr_offsets": [_vp, _P(_c.c_int), _P(_c.c_int)],
         "b200_offset_plan_i64": [_i64, _i64, _vp, _vp, _vp, _vp, _P(_c.c_int), _P(_c.c_int)],
         "b200_csr_narrow": [_vp, _P(_c.c_int)],
+        "b200_csr_value_bytes": [_vp, _P(_c.c_int)],
+        "b200_values_fit_f32": [_vp, _i64, _P(_c.c_int)],
         "b200_narrow_plan_i64": [_i64, _i64, _vp, _vp, _c.c_int, _c.c_int, _vp, _i64, _vp, _vp, _vp,
                                  _P(_i64), _P(_c.c_int)],
         "b200_csr_window": [_vp, _P(_c.c_int), _P(_c.c_int), _P(_c.c_int), _P(_i64)],
@@ -330,18 +332,19 @@ class Context:
         _check(lib().b200_profile_begin(self.h), "b200_profile_begin")
 
     def profile_end(self):
-        """Per (matrix shape, mode, column format) device times of the CSR kernels since
-        profile_begin()."""
+        """Per (matrix shape, mode, column format, value width) device times of the CSR kernels
+        since profile_begin(); value_bytes is 4 or 8 for a CSR pass, 0 for the other kernels."""
         cap = 256
         buf = (ProfileFormatEntry * cap)()
         cnt = _i64()
         _check(lib().b200_profile_end_formats(self.h, buf, cap, _c.byref(cnt)), "b200_profile_end_formats")
         out = []
         for i in range(min(cap, cnt.value)):
-            e, fmt = buf[i].entry, buf[i].format
+            e, fmt, vb = buf[i].entry, buf[i].format, buf[i].value_bytes
             out.append({"nrows": e.nrows, "ncols": e.ncols, "nnz": e.nnz,
                         "mode": MODE_NAMES.get(e.mode, str(e.mode)), "launches": e.launches,
-                        "total_ms": e.total_ms, "min_ms": e.min_ms, "format": FORMAT_NAMES[fmt]})
+                        "total_ms": e.total_ms, "min_ms": e.min_ms, "format": FORMAT_NAMES[fmt],
+                        "value_bytes": vb})
         return out
 
     def close(self):
@@ -570,6 +573,13 @@ class Csr:
         _check(lib().b200_csr_narrow(self.h, _c.byref(w)))
         return w.value
 
+    def value_bytes(self):
+        """Bytes per value the streaming passes read from this operator: 4 for an FP32 operator
+        and for an FP64 one whose values are all exact FP32, else 8 (b200_csr_value_bytes)."""
+        b = _c.c_int()
+        _check(lib().b200_csr_value_bytes(self.h, _c.byref(b)))
+        return b.value
+
     def window(self):
         """Windowed storage of this operator (include/amgcl_b200.h: b200_csr_window)."""
         w, ms, mr, tot = _c.c_int(), _c.c_int(), _c.c_int(), _i64()
@@ -640,6 +650,16 @@ def narrow_plan(nrows, ncols, ptr, col, lanes=0, nnz_cap=2048):
         if w.value == 24:
             out["hi8"] = hi8[:nnz]
     return out
+
+
+def values_fit_f32(val):
+    """Host-only: whether every value keeps its bits through double -> float -> double, the rule
+    b200_csr_create applies before it also stores an FP64 operator's values as FP32
+    (b200_values_fit_f32)."""
+    val = np.ascontiguousarray(val, dtype=np.float64)
+    ok = _c.c_int()
+    _check(lib().b200_values_fit_f32(val.ctypes.data, val.size, _c.byref(ok)))
+    return bool(ok.value)
 
 
 def window_plan(nrows, ncols, ptr, col, lanes=0, nnz_cap=2048, slot_cap=1400, max_ratio=75, gap=2):

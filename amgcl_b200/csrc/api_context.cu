@@ -91,6 +91,7 @@ extern "C" int b200_ctx_create(int device, b200_ctx_t *out) {
     if (const char *e = getenv("B200_OFFSETS")) ctx->opt_offsets = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_OFFSETS_MIN_NNZ")) ctx->opt_offsets_min_nnz = atoll(e);
     if (const char *e = getenv("B200_NARROW_COLUMNS")) ctx->opt_narrow = atoi(e) ? 1 : 0;
+    if (const char *e = getenv("B200_NARROW_VALUES")) ctx->opt_narrow_values = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_WINDOW")) ctx->opt_window = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_WINDOW_MIN_NNZ")) ctx->opt_window_min_nnz = atoll(e);
     if (const char *e = getenv("B200_WINDOW_GAP")) ctx->opt_window_gap = std::max(1, std::min(8, atoi(e)));
@@ -225,7 +226,7 @@ extern "C" int b200_profile_begin(b200_ctx_t ctx) {
     return B200_OK;
 }
 
-// per (shape, mode, format) device times of the launches since b200_profile_begin
+// per (shape, mode, format, value width) device times of the launches since b200_profile_begin
 static int profile_collect(b200_ctx_t ctx, std::vector<b200_profile_format_entry> &agg) {
     GUARD(ctx);
     ctx->profiling = false;
@@ -236,12 +237,12 @@ static int profile_collect(b200_ctx_t ctx, std::vector<b200_profile_format_entry
         b200_profile_format_entry *hit = nullptr;
         for (auto &a : agg)
             if (a.entry.nrows == r.nrows && a.entry.ncols == r.ncols && a.entry.nnz == r.nnz &&
-                a.entry.mode == r.mode && a.format == r.fmt) {
+                a.entry.mode == r.mode && a.format == r.fmt && a.value_bytes == r.vbytes) {
                 hit = &a;
                 break;
             }
         if (!hit) {
-            agg.push_back({{r.nrows, r.ncols, r.nnz, r.mode, 0, 0.0, 1e30}, r.fmt});
+            agg.push_back({{r.nrows, r.ncols, r.nnz, r.mode, 0, 0.0, 1e30}, r.fmt, r.vbytes});
             hit = &agg.back();
         }
         hit->entry.launches += 1;
@@ -306,6 +307,8 @@ static int64_t *option_slot(b200_ctx_t ctx, const char *key) {
     if (!strcmp(key, "offsets")) return &ctx->opt_offsets;
     if (!strcmp(key, "offsets_min_nnz")) return &ctx->opt_offsets_min_nnz;
     if (!strcmp(key, "narrow_columns")) return &ctx->opt_narrow;
+    if (!strcmp(key, "narrow_values")) return &ctx->opt_narrow_values;
+    if (!strcmp(key, "narrow_values_min_nnz")) return &ctx->opt_narrow_values_min_nnz;
     if (!strcmp(key, "window")) return &ctx->opt_window;
     if (!strcmp(key, "window_min_nnz")) return &ctx->opt_window_min_nnz;
     if (!strcmp(key, "window_ratio")) return &ctx->opt_window_ratio;

@@ -136,6 +136,23 @@ static cudaError_t staged_upload(b200_ctx_t ctx, Dst *dst, const Src *src, size_
     return rc;
 }
 
+// Do all n values keep their exact bits through double -> float -> double?  (Pure host logic, also
+// exported as b200_values_fit_f32 for tests.)  Bits, not ==: -0.0 must stay -0.0, and a NaN
+// qualifies only if its payload survives.  A float subnormal lost to rounding, a double subnormal
+// or a value beyond FLT_MAX does not come back.
+static bool values_fit_f32(const double *val, int64_t n) {
+    int bad = 0;
+#pragma omp parallel for reduction(| : bad) schedule(static)
+    for (int64_t e = 0; e < n; ++e) {
+        const double w = (double)(float)val[e];
+        uint64_t a, b;
+        memcpy(&a, val + e, 8);
+        memcpy(&b, &w, 8);
+        bad |= a != b ? 1 : 0;
+    }
+    return !bad;
+}
+
 // Upload one CSR matrix exactly as the kernels will see it (indices narrowed to int32,
 // row-block plan built).  Single-GPU matrices come straight through here; the
 // distributed kinds hand in the local part produced by dist.cuh.
@@ -221,6 +238,11 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     const bool narrowed = !pattern_indexed && !offset_indexed && !windowed && ctx->opt_narrow && nlong == 0 &&
                           lanes <= 8 && build_narrow(blk4.data(), nblocks, col, nnz, nar);
 
+    // ---- FP32 copy of the values of an FP64 operator that loses nothing in FP32 ----------------
+    bool values32 = false;
+    if constexpr (std::is_same<Val, double>::value)
+        values32 = ctx->opt_narrow_values && nnz >= ctx->opt_narrow_values_min_nnz && values_fit_f32(val, nnz);
+
     // ---- block-relative row pointers of the final blocks --------------------------------
     std::vector<unsigned short> ptr16((size_t)nrows, 0);
     build_ptr16(blk4.data(), nblocks, hptr.data(), nnz_cap, ptr16);
@@ -248,6 +270,7 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     const size_t ptr_bytes = ((size_t)nrows + 1 + 8) * sizeof(int);
     const size_t col_bytes = ((size_t)nnz + 8) * sizeof(int);
     const size_t val_bytes = ((size_t)nnz + 8) * sizeof(Val);
+    const size_t v32_bytes = values32 ? ((size_t)nnz + 8) * sizeof(float) : 0;
     const size_t blk_bytes = ((size_t)nblocks + 1) * sizeof(int4);
     const size_t c16_bytes = windowed ? ((size_t)nnz + 16) * sizeof(unsigned short) : 0;
     const size_t run_bytes = windowed ? (win.runs.size() + 4) * sizeof(int2) : 0;
@@ -264,6 +287,7 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
         if (A->ptr) cudaFree(A->ptr);
         if (A->col) cudaFree(A->col);
         if (A->val) cudaFree(A->val);
+        if (A->val32) cudaFree(A->val32);
         if (A->blk) cudaFree(A->blk);
         if (A->col16) cudaFree(A->col16);
         if (A->wrun) cudaFree(A->wrun);
@@ -298,6 +322,11 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     if (nnz) {
         CSR_CUDA(staged_upload(ctx, A->col, col, (size_t)nnz));      // narrowed to int32 on the way
         CSR_CUDA(staged_upload(ctx, static_cast<Val *>(A->val), val, (size_t)nnz));
+    }
+    if (values32) {
+        CSR_CUDA(cudaMalloc(&A->val32, v32_bytes));
+        CSR_CUDA(cudaMemsetAsync(A->val32, 0, v32_bytes, ctx->stream));
+        CSR_CUDA(staged_upload(ctx, A->val32, val, (size_t)nnz));     // exact: checked above
     }
     CSR_CUDA(cudaMemcpyAsync(A->blk, blk4.data(), blk_bytes, cudaMemcpyHostToDevice, ctx->stream));
     CSR_CUDA(cudaMalloc(&A->ptr16, p16_bytes));
@@ -352,7 +381,7 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     }
     CSR_CUDA(cudaStreamSynchronize(ctx->stream));   // host staging buffers die here
 #undef CSR_CUDA
-    A->bytes = ptr_bytes + col_bytes + val_bytes + blk_bytes + c16_bytes + run_bytes + wbk_bytes + ix8_bytes +
+    A->bytes = ptr_bytes + col_bytes + val_bytes + v32_bytes + blk_bytes + c16_bytes + run_bytes + wbk_bytes + ix8_bytes +
                tab_bytes + pid_bytes + pat_bytes + p16_bytes + lo_bytes + hi_bytes + cb_bytes;
     if (nnz > ctx->big_nnz) {
         ctx->big_nnz = nnz;
@@ -367,6 +396,7 @@ static void csr_free(b200_csr_t A) {
     if (A->ptr) cudaFree(A->ptr);
     if (A->col) cudaFree(A->col);
     if (A->val) cudaFree(A->val);
+    if (A->val32) cudaFree(A->val32);
     if (A->blk) cudaFree(A->blk);
     if (A->col16) cudaFree(A->col16);
     if (A->wrun) cudaFree(A->wrun);
@@ -553,6 +583,20 @@ static int launch_csr_L(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {
 }
 
 template <int MODE, class P>
+static int launch_csr_lanes(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {
+    if (ctx->recording) A->in_graph = true;
+    ProfScope prof(ctx, MODE, A->nrows, A->ncols, A->nnz, launch_format<P>(ctx, A), (int)sizeof(typename P::TV));
+    switch (A->lanes) {
+    case 1:  return launch_csr_L<MODE, 1>(ctx, A, args);
+    case 2:  return launch_csr_L<MODE, 2>(ctx, A, args);
+    case 4:  return launch_csr_L<MODE, 4>(ctx, A, args);
+    case 8:  return launch_csr_L<MODE, 8>(ctx, A, args);
+    case 16: return launch_csr_L<MODE, 16>(ctx, A, args);
+    default: return launch_csr_L<MODE, 32>(ctx, A, args);
+    }
+}
+
+template <int MODE, class P>
 static int launch_csr(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {
     if (A->nblocks == 0) return B200_OK;
     // small FP64 operator, nothing to reduce or exchange: defer into the coarse-tail list
@@ -567,16 +611,18 @@ static int launch_csr(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {
     if (std::is_same<P, PrecDD>::value && MODE != MODE_RESID_SCALED && !args.ndot && !args.xh &&
         !args.gather_on && small_csr_accepts(ctx, A))
         return small_csr_launch(ctx, MODE, A, *reinterpret_cast<const CsrArgsT<PrecDD> *>(&args));
-    if (ctx->recording) A->in_graph = true;
-    ProfScope prof(ctx, MODE, A->nrows, A->ncols, A->nnz, launch_format<P>(ctx, A));
-    switch (A->lanes) {
-    case 1:  return launch_csr_L<MODE, 1>(ctx, A, args);
-    case 2:  return launch_csr_L<MODE, 2>(ctx, A, args);
-    case 4:  return launch_csr_L<MODE, 4>(ctx, A, args);
-    case 8:  return launch_csr_L<MODE, 8>(ctx, A, args);
-    case 16: return launch_csr_L<MODE, 16>(ctx, A, args);
-    default: return launch_csr_L<MODE, 32>(ctx, A, args);
+    if constexpr (std::is_same<P, PrecDD>::value) {
+        // the ring kernel streams the FP32 copy of an operator whose values are all exact FP32
+        // (the cross-check variant, the tail and the small-operator kernel read the FP64 values)
+        if (A->val32 && ctx->opt_narrow_values && ctx->opt_spmv_variant == 1) {
+            CsrArgsT<PrecSD> s;
+            static_assert(sizeof(s) == sizeof(args), "PrecSD arguments differ from PrecDD only in the value type");
+            memcpy(&s, &args, sizeof(s));
+            s.val = A->val32;
+            return launch_csr_lanes<MODE>(ctx, A, s);
+        }
     }
+    return launch_csr_lanes<MODE>(ctx, A, args);
 }
 
 template <class P>
@@ -829,6 +875,18 @@ extern "C" int b200_csr_offsets(b200_csr_t A, int *offset_indexed, int *count) {
 extern "C" int b200_csr_narrow(b200_csr_t A, int *width) {
     B200_REQUIRE(A && width, "null argument");
     *width = A->narrow;
+    return B200_OK;
+}
+
+extern "C" int b200_csr_value_bytes(b200_csr_t A, int *bytes) {
+    B200_REQUIRE(A && bytes, "null argument");
+    *bytes = A->val32 || A->dtype == B200_F32 ? 4 : 8;
+    return B200_OK;
+}
+
+extern "C" int b200_values_fit_f32(const double *val, int64_t n, int *qualifies) {
+    B200_REQUIRE(n >= 0 && (val || n == 0) && qualifies, "bad argument");
+    *qualifies = values_fit_f32(val, n) ? 1 : 0;
     return B200_OK;
 }
 

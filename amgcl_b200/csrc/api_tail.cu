@@ -105,7 +105,7 @@ int small_csr_launch(b200_ctx_t ctx, int mode, b200_csr_t A, const CsrArgsT<Prec
     const int64_t want = ((int64_t)A->nrows * A->lanes + kThreads - 1) / kThreads;
     const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)ctx->sm_count * 8));
     if (ctx->recording) A->in_graph = true;
-    ProfScope prof(ctx, mode, A->nrows, A->ncols, A->nnz);
+    ProfScope prof(ctx, mode, A->nrows, A->ncols, A->nnz, 0, (int)sizeof(double));
     cudaError_t rc;
     switch (A->lanes) {
     case 1:  rc = launch_pdl(ctx, small_csr_kernel<1>, dim3(grid), dim3(kThreads), 0, c); break;

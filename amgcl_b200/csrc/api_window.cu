@@ -34,5 +34,10 @@ B200_WIN_INST(MODE_RESID_SCALED, PrecDD)
 B200_WIN_INST(MODE_RELAX, PrecDD)
 B200_WIN_INST(MODE_RELAX, PrecFF)
 B200_WIN_INST(MODE_RELAX, PrecFD)
+B200_WIN_INST(MODE_SPMV, PrecSD)
+B200_WIN_INST(MODE_SPMV_ACC, PrecSD)
+B200_WIN_INST(MODE_RESID, PrecSD)
+B200_WIN_INST(MODE_RESID_SCALED, PrecSD)
+B200_WIN_INST(MODE_RELAX, PrecSD)
 
 } // namespace b200

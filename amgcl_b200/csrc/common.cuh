@@ -123,7 +123,7 @@ struct b200_ctx_s {
     bool                      profiling = false;
     std::vector<cudaEvent_t>  prof_events;      // pool, used pairwise
     size_t                    prof_used = 0;
-    struct ProfRec { int64_t nrows, ncols, nnz; int mode; size_t ev; int fmt; };
+    struct ProfRec { int64_t nrows, ncols, nnz; int mode; size_t ev; int fmt, vbytes; };
     std::vector<ProfRec>      prof_recs;
 
     // multi-GPU (dist.cuh): one process per GPU, this context's share of the job
@@ -166,6 +166,8 @@ struct b200_ctx_s {
     int64_t opt_offsets       = 1;        // operators with <= 256 distinct (col - row): 8-bit column indices
     int64_t opt_offsets_min_nnz = 1000000;// ... from this many non-zeros on (decided at upload)
     int64_t opt_narrow        = 1;        // other operators: 16- or 24-bit block-relative columns (narrow.cuh)
+    int64_t opt_narrow_values = 1;        // FP64 operators whose values are all exact FP32: stream 4-byte values
+    int64_t opt_narrow_values_min_nnz = 1000000;   // ... from this many non-zeros on (decided at upload)
     int64_t opt_window        = 0;        // operators that qualify gather x through shared-memory windows
     int64_t opt_window_min_nnz = 1000000; // ... "qualify": at least this many non-zeros (decided at upload),
     int64_t opt_window_ratio  = 75;       // ... windows no larger than this percentage of the entries,
@@ -250,6 +252,8 @@ struct b200_csr_s {
     int       *ptr   = nullptr;   // [nrows+1] (+ padding) device
     int       *col   = nullptr;   // [nnz]     (+ padding) device
     void      *val   = nullptr;   // [nnz]     (+ padding) device, FP64 or FP32
+    float     *val32 = nullptr;   // [nnz]     (+ padding) FP64 operator whose every value is exactly an FP32:
+                                  //   the values the ring kernel streams (same bits once widened)
     int        dtype = B200_F64;
     double    *scratch64 = nullptr;   // FP32 operator swept on FP64 vectors: new iterate
     bool       in_graph  = false;     // some recorded graph refers to this operator

@@ -69,7 +69,9 @@
 // combinations are the ones AMGCL's mixed-precision composition produces (FP32
 // hierarchy under an FP64 Krylov solver, tutorial/1.poisson3Db/poisson3Db.cpp:45-51):
 // as in the reference (matrix_ops.hpp:57) a row sum is accumulated in the value
-// type of the OUTPUT vector.
+// type of the OUTPUT vector.  An FP64 operator whose every value converts to FP32 and back
+// with the same bits also streams them as FP32 (PrecSD): the widened value is the same double,
+// so every product, row sum and epilogue is that of PrecDD.
 #pragma once
 #include "common.cuh"
 #include "reduce.cuh"
@@ -112,6 +114,9 @@ typedef Prec<float, float, float, float, float>      PrecFF;   // FP32 level of 
 typedef Prec<float, double, double, double, float>   PrecFD;   // FP32 operator on FP64 vectors
 typedef Prec<float, double, double, float, float>    PrecFDF;  // finest residual into FP32 scratch
 typedef Prec<float, float, float, double, float>     PrecFFD;  // prolongation into an FP64 iterate
+// FP64 operator whose values are all exact FP32 (b200_csr_s::val32): 4-byte values widened to the
+// same doubles at FMA time, FP64 everything else -- the bits of PrecDD
+typedef Prec<float, double, double, double, double>  PrecSD;
 
 template <class P>
 struct CsrArgsT {

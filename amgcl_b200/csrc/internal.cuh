@@ -44,8 +44,9 @@ struct ProfScope {
     int64_t nrows, ncols, nnz;
     int mode;
     int fmt;            // CSR passes: the column format streamed (FMT_*)
-    ProfScope(b200_ctx_t c, int mode_, int64_t nr, int64_t nc, int64_t nz, int fmt_ = 0)
-        : ctx(c), nrows(nr), ncols(nc), nnz(nz), mode(mode_), fmt(fmt_) {
+    int vbytes;         // ... and the bytes of one stored value (0 for the other kernels)
+    ProfScope(b200_ctx_t c, int mode_, int64_t nr, int64_t nc, int64_t nz, int fmt_ = 0, int vbytes_ = 0)
+        : ctx(c), nrows(nr), ncols(nc), nnz(nz), mode(mode_), fmt(fmt_), vbytes(vbytes_) {
         if (!ctx->profiling || ctx->prof_recs.size() >= kProfMaxPairs) return;
         while (ctx->prof_events.size() < ctx->prof_used + 2) {
             cudaEvent_t e;
@@ -60,7 +61,7 @@ struct ProfScope {
         if (!on) return;
         if (cudaEventRecord(ctx->prof_events[ev + 1], ctx->stream) != cudaSuccess) return;
         ctx->prof_used += 2;
-        ctx->prof_recs.push_back({nrows, ncols, nnz, mode, ev, fmt});
+        ctx->prof_recs.push_back({nrows, ncols, nnz, mode, ev, fmt, vbytes});
     }
 };
 

@@ -41,11 +41,27 @@ int b200_narrow_plan_i64(int64_t nrows, int64_t ncols, const int64_t *ptr, const
                          int nnz_cap, int32_t *base_out, int64_t base_capacity, uint16_t *lo16_out,
                          uint8_t *hi8_out, uint16_t *ptr16_out, int64_t *nblocks_out, int *width_out);
 
-/* b200_profile_end with the column format each CSR pass streamed (B200_FMT_*; 0 for the other
- * kernels).  Entries are aggregated per (shape, mode, format). */
+/* Narrow values.  An FP64 operator with at least "narrow_values_min_nnz" non-zeros (default 1e6)
+ * whose every value has the same bits after double -> float -> double (integer and dyadic
+ * stencils, graph Laplacians, matrices assembled from FP32 data) also stores its values as FP32,
+ * and the streaming passes read 4 instead of 8 bytes per value.  The widened value is the same
+ * double, so every product, row sum and result keeps its bits.  The FP64 values stay: the
+ * one-block-per-CTA variant (spmv_variant 0), the small-operator kernel and the coarse tail read
+ * them.  Context option "narrow_values" (b200_ctx_set_option; env B200_NARROW_VALUES): 1 = built
+ * at upload and used (default), 0 = not built / not used.
+ * b200_csr_value_bytes: 4 or 8, the bytes per value the streaming passes read from A.
+ * b200_values_fit_f32: pure host helper for tests, the rule b200_csr_create applies to n values
+ * (qualifies 1: every value survives the round trip). */
+int b200_csr_value_bytes(b200_csr_t A, int *bytes);
+int b200_values_fit_f32(const double *val, int64_t n, int *qualifies);
+
+/* b200_profile_end with the column format (B200_FMT_*) and the bytes per stored value (4 or 8)
+ * each CSR pass streamed (0 and 0 for the other kernels).  Entries are aggregated per
+ * (shape, mode, format, value width). */
 typedef struct {
     b200_profile_entry entry;
     int                format;
+    int                value_bytes;
 } b200_profile_format_entry;
 int b200_profile_end_formats(b200_ctx_t ctx, b200_profile_format_entry *out, int64_t capacity,
                              int64_t *count);
