@@ -152,6 +152,7 @@ def lib():
         "b200_csr_narrow": [_vp, _P(_c.c_int)],
         "b200_csr_value_bytes": [_vp, _P(_c.c_int)],
         "b200_values_fit_f32": [_vp, _i64, _P(_c.c_int)],
+        "b200_value_index_plan_i64": [_vp, _i64, _vp, _i64, _vp, _P(_c.c_int), _P(_c.c_int)],
         "b200_narrow_plan_i64": [_i64, _i64, _vp, _vp, _c.c_int, _c.c_int, _vp, _i64, _vp, _vp, _vp,
                                  _P(_i64), _P(_c.c_int)],
         "b200_csr_window": [_vp, _P(_c.c_int), _P(_c.c_int), _P(_c.c_int), _P(_i64)],
@@ -333,7 +334,7 @@ class Context:
 
     def profile_end(self):
         """Per (matrix shape, mode, column format, value width) device times of the CSR kernels
-        since profile_begin(); value_bytes is 4 or 8 for a CSR pass, 0 for the other kernels."""
+        since profile_begin(); value_bytes is 1, 2, 4 or 8 for a CSR pass, 0 for the other kernels."""
         cap = 256
         buf = (ProfileFormatEntry * cap)()
         cnt = _i64()
@@ -575,7 +576,8 @@ class Csr:
 
     def value_bytes(self):
         """Bytes per value the streaming passes read from this operator: 4 for an FP32 operator
-        and for an FP64 one whose values are all exact FP32, else 8 (b200_csr_value_bytes)."""
+        and for an FP64 one whose values are all exact FP32, 1 or 2 for an FP64 one streamed as
+        indices into the table of its distinct values, else 8 (b200_csr_value_bytes)."""
         b = _c.c_int()
         _check(lib().b200_csr_value_bytes(self.h, _c.byref(b)))
         return b.value
@@ -660,6 +662,23 @@ def values_fit_f32(val):
     ok = _c.c_int()
     _check(lib().b200_values_fit_f32(val.ctypes.data, val.size, _c.byref(ok)))
     return bool(ok.value)
+
+
+def value_index_plan(val):
+    """Host-only: the index into the table of distinct values that b200_csr_create builds for an
+    FP64 operator (b200_value_index_plan_i64).  Returns {"width": 8 or 16, "count", "table",
+    "index"}, or {"width": 0, "count": 4097} when there are more than 4,096 distinct values."""
+    val = np.ascontiguousarray(val, dtype=np.float64)
+    tab = np.zeros(4096, dtype=np.float64)
+    idx = np.zeros(max(1, 2 * val.size), dtype=np.uint8)
+    cnt, w = _c.c_int(), _c.c_int()
+    _check(lib().b200_value_index_plan_i64(val.ctypes.data, val.size, tab.ctypes.data, tab.size,
+                                            idx.ctypes.data, _c.byref(cnt), _c.byref(w)))
+    out = {"width": w.value, "count": cnt.value}
+    if w.value:
+        out["table"] = tab[:cnt.value]
+        out["index"] = idx[:val.size] if w.value == 8 else idx[:2 * val.size].view(np.uint16)
+    return out
 
 
 def window_plan(nrows, ncols, ptr, col, lanes=0, nnz_cap=2048, slot_cap=1400, max_ratio=75, gap=2):

@@ -9,6 +9,7 @@
 #include "offsets.cuh"
 #include "patterns.cuh"
 #include "narrow.cuh"
+#include "values.cuh"
 
 namespace b200 {
 int tail_enqueue_csr(b200_ctx_t ctx, int mode, b200_csr_t A, const CsrArgsT<PrecDD> &a);   // api_tail.cu
@@ -243,6 +244,18 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     if constexpr (std::is_same<Val, double>::value)
         values32 = ctx->opt_narrow_values && nnz >= ctx->opt_narrow_values_min_nnz && values_fit_f32(val, nnz);
 
+    // ---- otherwise an index into the table of its distinct values (values.cuh), where the
+    // table fits beside the configured ring of the format the operator is streamed in -----------
+    ValueIndexPlan vip;
+    bool indexed = false;
+    if constexpr (std::is_same<Val, double>::value) {
+        const int fmt = pattern_indexed ? FMT_PATTERN : offset_indexed ? FMT_OFFSET
+                      : narrowed ? (nar.width == 24 ? FMT_COL24 : FMT_COL16) : FMT_PLAIN;
+        indexed = !values32 && ctx->opt_narrow_values && nnz > 0 && nnz >= ctx->opt_narrow_values_min_nnz &&
+                  nlong == 0 && !windowed && !ctx->dist && build_value_index(val, nnz, vip) &&
+                  value_index_fits(ctx, rows_cap, nnz_cap, fmt, vip.width / 8, vip.count);
+    }
+
     // ---- block-relative row pointers of the final blocks --------------------------------
     std::vector<unsigned short> ptr16((size_t)nrows, 0);
     build_ptr16(blk4.data(), nblocks, hptr.data(), nnz_cap, ptr16);
@@ -271,6 +284,8 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     const size_t col_bytes = ((size_t)nnz + 8) * sizeof(int);
     const size_t val_bytes = ((size_t)nnz + 8) * sizeof(Val);
     const size_t v32_bytes = values32 ? ((size_t)nnz + 8) * sizeof(float) : 0;
+    const size_t vix_bytes = indexed ? (((size_t)nnz + 32) * (size_t)(vip.width / 8) + 15) & ~(size_t)15 : 0;
+    const size_t vtb_bytes = indexed ? (size_t)vip.count * sizeof(double) : 0;
     const size_t blk_bytes = ((size_t)nblocks + 1) * sizeof(int4);
     const size_t c16_bytes = windowed ? ((size_t)nnz + 16) * sizeof(unsigned short) : 0;
     const size_t run_bytes = windowed ? (win.runs.size() + 4) * sizeof(int2) : 0;
@@ -288,6 +303,8 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
         if (A->col) cudaFree(A->col);
         if (A->val) cudaFree(A->val);
         if (A->val32) cudaFree(A->val32);
+        if (A->vidx) cudaFree(A->vidx);
+        if (A->vtab) cudaFree(A->vtab);
         if (A->blk) cudaFree(A->blk);
         if (A->col16) cudaFree(A->col16);
         if (A->wrun) cudaFree(A->wrun);
@@ -327,6 +344,16 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
         CSR_CUDA(cudaMalloc(&A->val32, v32_bytes));
         CSR_CUDA(cudaMemsetAsync(A->val32, 0, v32_bytes, ctx->stream));
         CSR_CUDA(staged_upload(ctx, A->val32, val, (size_t)nnz));     // exact: checked above
+    }
+    if (indexed) {
+        CSR_CUDA(cudaMalloc(&A->vidx, vix_bytes));
+        CSR_CUDA(cudaMalloc(&A->vtab, vtb_bytes));
+        CSR_CUDA(cudaMemsetAsync(A->vidx, 0, vix_bytes, ctx->stream));
+        if (vip.width == 8) CSR_CUDA(staged_upload(ctx, static_cast<unsigned char *>(A->vidx), vip.idx8.data(), (size_t)nnz));
+        else CSR_CUDA(staged_upload(ctx, static_cast<unsigned short *>(A->vidx), vip.idx16.data(), (size_t)nnz));
+        CSR_CUDA(staged_upload(ctx, reinterpret_cast<uint64_t *>(A->vtab), vip.tab.data(), (size_t)vip.count));
+        A->vidx_bytes = vip.width / 8;
+        A->vtab_n = vip.count;
     }
     CSR_CUDA(cudaMemcpyAsync(A->blk, blk4.data(), blk_bytes, cudaMemcpyHostToDevice, ctx->stream));
     CSR_CUDA(cudaMalloc(&A->ptr16, p16_bytes));
@@ -381,7 +408,7 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     }
     CSR_CUDA(cudaStreamSynchronize(ctx->stream));   // host staging buffers die here
 #undef CSR_CUDA
-    A->bytes = ptr_bytes + col_bytes + val_bytes + v32_bytes + blk_bytes + c16_bytes + run_bytes + wbk_bytes + ix8_bytes +
+    A->bytes = ptr_bytes + col_bytes + val_bytes + v32_bytes + vix_bytes + vtb_bytes + blk_bytes + c16_bytes + run_bytes + wbk_bytes + ix8_bytes +
                tab_bytes + pid_bytes + pat_bytes + p16_bytes + lo_bytes + hi_bytes + cb_bytes;
     if (nnz > ctx->big_nnz) {
         ctx->big_nnz = nnz;
@@ -397,6 +424,8 @@ static void csr_free(b200_csr_t A) {
     if (A->col) cudaFree(A->col);
     if (A->val) cudaFree(A->val);
     if (A->val32) cudaFree(A->val32);
+    if (A->vidx) cudaFree(A->vidx);
+    if (A->vtab) cudaFree(A->vtab);
     if (A->blk) cudaFree(A->blk);
     if (A->col16) cudaFree(A->col16);
     if (A->wrun) cudaFree(A->wrun);
@@ -554,11 +583,13 @@ static int launch_csr_LH(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) 
                 done = true;
             }
         }
-        if constexpr (L <= 8) {
+        if constexpr (L <= 8 && !IndexedValues<typename P::TV>::value) {   // (indexed: never windowed)
             if (fmt == FMT_WINDOW) {
                 rc = launch_ring_win<MODE, L, HALO, P>(ctx, A, args);
                 done = true;
             }
+        }
+        if constexpr (L <= 8) {
             if (fmt == FMT_COL16) {
                 rc = launch_ring_c16<MODE, L, HALO, P>(ctx, A, args);
                 done = true;
@@ -578,7 +609,9 @@ static int launch_csr_LH(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) 
 
 template <int MODE, int L, class P>
 static int launch_csr_L(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {
-    if (args.xh) return launch_csr_LH<MODE, L, true, P>(ctx, A, args);
+    if constexpr (!IndexedValues<typename P::TV>::value) {   // (indexed: single-GPU contexts only)
+        if (args.xh) return launch_csr_LH<MODE, L, true, P>(ctx, A, args);
+    }
     return launch_csr_LH<MODE, L, false, P>(ctx, A, args);
 }
 
@@ -594,6 +627,18 @@ static int launch_csr_lanes(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &arg
     case 16: return launch_csr_L<MODE, 16>(ctx, A, args);
     default: return launch_csr_L<MODE, 32>(ctx, A, args);
     }
+}
+
+// the arguments of an FP64 pass, streaming A's value index instead of its values
+template <class PI>
+static CsrArgsT<PI> indexed_args(b200_csr_t A, const CsrArgsT<PrecDD> &args) {
+    CsrArgsT<PI> s;
+    static_assert(sizeof(s) == sizeof(args), "indexed arguments differ from PrecDD only in the value type");
+    memcpy(&s, &args, sizeof(s));
+    s.val = static_cast<const typename PI::TV *>(A->vidx);
+    s.vtab = A->vtab;
+    s.vtab_n = A->vtab_n;
+    return s;
 }
 
 template <int MODE, class P>
@@ -620,6 +665,13 @@ static int launch_csr(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {
             memcpy(&s, &args, sizeof(s));
             s.val = A->val32;
             return launch_csr_lanes<MODE>(ctx, A, s);
+        }
+        // ... or the 8- / 16-bit index of an operator with few distinct values, as long as the table
+        // fits beside the configured ring (options may have changed since the upload)
+        if (A->vidx && ctx->opt_narrow_values && ctx->opt_spmv_variant == 1 &&
+            value_index_fits(ctx, A->rows_cap, A->nnz_cap, launch_format<PrecDD>(ctx, A), A->vidx_bytes, A->vtab_n)) {
+            if (A->vidx_bytes == 1) return launch_csr_lanes<MODE>(ctx, A, indexed_args<PrecI8D>(A, args));
+            return launch_csr_lanes<MODE>(ctx, A, indexed_args<PrecI16D>(A, args));
         }
     }
     return launch_csr_lanes<MODE>(ctx, A, args);
@@ -880,7 +932,26 @@ extern "C" int b200_csr_narrow(b200_csr_t A, int *width) {
 
 extern "C" int b200_csr_value_bytes(b200_csr_t A, int *bytes) {
     B200_REQUIRE(A && bytes, "null argument");
-    *bytes = A->val32 || A->dtype == B200_F32 ? 4 : 8;
+    *bytes = A->val32 || A->dtype == B200_F32 ? 4 : A->vidx ? A->vidx_bytes : 8;
+    return B200_OK;
+}
+
+extern "C" int b200_value_index_plan_i64(const double *val, int64_t n, double *table_out, int64_t table_capacity,
+                                         void *idx_out, int *count_out, int *width_out) {
+    B200_REQUIRE(n >= 0 && (val || n == 0) && count_out && width_out, "bad argument");
+    ValueIndexPlan p;
+    const bool ok = build_value_index(val, n, p);
+    *count_out = p.count;
+    *width_out = ok ? p.width : 0;
+    if (!ok) return B200_OK;
+    if (table_out) {
+        B200_REQUIRE(table_capacity >= p.count, "table_out too small");
+        memcpy(table_out, p.tab.data(), (size_t)p.count * sizeof(double));
+    }
+    if (idx_out && n) {
+        if (p.width == 8) memcpy(idx_out, p.idx8.data(), (size_t)n);
+        else memcpy(idx_out, p.idx16.data(), (size_t)n * 2);
+    }
     return B200_OK;
 }
 

@@ -40,4 +40,14 @@ B200_OFF_INST(MODE_RESID, PrecSD)
 B200_OFF_INST(MODE_RESID_SCALED, PrecSD)
 B200_OFF_INST(MODE_RELAX, PrecSD)
 
+// indexed values (PrecI8D / PrecI16D): single-GPU only, so without the halo
+#define B200_OFF_IDX_L(MODE, L, P)                                                                   \
+    template int launch_ring_off<MODE, L, false, P>(b200_ctx_t, b200_csr_t, const CsrArgsT<P> &);
+#define B200_OFF_IDX(MODE, P) B200_OFF_IDX_L(MODE, 1, P) B200_OFF_IDX_L(MODE, 2, P) B200_OFF_IDX_L(MODE, 4, P)
+#define B200_OFF_IDX_P(P)                                                                             \
+    B200_OFF_IDX(MODE_SPMV, P) B200_OFF_IDX(MODE_SPMV_ACC, P) B200_OFF_IDX(MODE_RESID, P)                 \
+    B200_OFF_IDX(MODE_RESID_SCALED, P) B200_OFF_IDX(MODE_RELAX, P)
+B200_OFF_IDX_P(PrecI8D)
+B200_OFF_IDX_P(PrecI16D)
+
 } // namespace b200

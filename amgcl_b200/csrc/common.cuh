@@ -254,6 +254,10 @@ struct b200_csr_s {
     void      *val   = nullptr;   // [nnz]     (+ padding) device, FP64 or FP32
     float     *val32 = nullptr;   // [nnz]     (+ padding) FP64 operator whose every value is exactly an FP32:
                                   //   the values the ring kernel streams (same bits once widened)
+    void      *vidx  = nullptr;   // [nnz]     (+ padding) FP64 operator with few distinct values: 8- or
+    double    *vtab  = nullptr;   //   16-bit index of every value in vtab [vtab_n], the distinct values
+    int        vidx_bytes = 0;    //   sorted by bit pattern (values.cuh); the values the ring kernel
+    int        vtab_n     = 0;    //   streams where the table fits beside the ring
     int        dtype = B200_F64;
     double    *scratch64 = nullptr;   // FP32 operator swept on FP64 vectors: new iterate
     bool       in_graph  = false;     // some recorded graph refers to this operator

@@ -71,7 +71,10 @@
 // as in the reference (matrix_ops.hpp:57) a row sum is accumulated in the value
 // type of the OUTPUT vector.  An FP64 operator whose every value converts to FP32 and back
 // with the same bits also streams them as FP32 (PrecSD): the widened value is the same double,
-// so every product, row sum and epilogue is that of PrecDD.
+// so every product, row sum and epilogue is that of PrecDD.  An FP64 operator with at most 4,096
+// distinct values streams an 8- or 16-bit index per entry instead (PrecI8D / PrecI16D, built by
+// values.cuh): the kernel reads the double the index names from a table in shared memory, so it
+// too multiplies the very same doubles as PrecDD.
 #pragma once
 #include "common.cuh"
 #include "reduce.cuh"
@@ -117,6 +120,23 @@ typedef Prec<float, float, float, double, float>     PrecFFD;  // prolongation i
 // FP64 operator whose values are all exact FP32 (b200_csr_s::val32): 4-byte values widened to the
 // same doubles at FMA time, FP64 everything else -- the bits of PrecDD
 typedef Prec<float, double, double, double, double>  PrecSD;
+// FP64 operator with at most 256 / 4,096 distinct values (b200_csr_s::vidx): the stage holds an
+// 8- / 16-bit index per entry, read as vtab[index] at FMA time -- the bits of PrecDD
+typedef Prec<unsigned char, double, double, double, double>  PrecI8D;
+typedef Prec<unsigned short, double, double, double, double> PrecI16D;
+
+// does the stored value type index a table of values?
+template <class TV> struct IndexedValues : std::false_type {};
+template <> struct IndexedValues<unsigned char> : std::true_type {};
+template <> struct IndexedValues<unsigned short> : std::true_type {};
+
+// the value of a stored entry, in the type of the row sum: the entry itself or, indexed, the
+// table entry it names
+template <class TS, class TV>
+__device__ __forceinline__ TS value_of(TV v, const double *vtab) {
+    if constexpr (IndexedValues<TV>::value) return (TS)vtab[v];
+    else return (TS)v;
+}
 
 template <class P>
 struct CsrArgsT {
@@ -124,6 +144,8 @@ struct CsrArgsT {
     const unsigned short *ptr16;   // staged blocks: ptr[r] - first non-zero of r's block
     const int    *col;
     const typename P::TV *val;
+    const double *vtab;   // indexed values: the table val indexes (vtab_n entries), else nullptr
+    int           vtab_n;
     const int4   *blk;    // [nblocks] in WALK ORDER: {first row (~first row if the block gathers
                           //   halo columns), end row, first non-zero, end non-zero}
     int           nrows;
@@ -233,8 +255,12 @@ constexpr int kWinRunLen   = 64;    // longest run of a window (longer ones are 
 constexpr int kOffTabLen   = 256;   // offset-indexed operators: entries of the (col - row) table
 constexpr int kPatCap      = 256;   // pattern-indexed operators: most row patterns ...
 constexpr int kPatOffCap   = 1024;  // ... and most offsets in all patterns together
-// shared memory behind the stages: the window of x / the offset table / the pattern tables
+// shared memory behind the stages: the window of x / the offset table / the pattern tables,
+// then an indexed operator's table of values
 constexpr int kPatTabBytes = kPatOffCap * 4 + ((kPatCap + 1) * 2 + 15) / 16 * 16;
+__host__ __device__ constexpr int fmt_table_bytes(int fmt) {   // (not FMT_WINDOW: sized per operator)
+    return fmt == FMT_OFFSET ? kOffTabLen * 4 : fmt == FMT_PATTERN ? kPatTabBytes : 0;
+}
 
 struct BlockDesc {      // written by the producer thread, read by everyone after the wait
     int r0, r1;         // row range
@@ -473,7 +499,8 @@ template <int MODE, int L, bool HALO, class P, int FMT = FMT_PLAIN>
 __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const BlockDesc &d,
                                                const char *stage, const StageLayout &lay, RowAcc &acc,
                                                const typename P::TX *win = nullptr, const int *off = nullptr,
-                                               const unsigned short *pstart = nullptr, int k0 = 0) {
+                                               const unsigned short *pstart = nullptr, int k0 = 0,
+                                               const double *vtab = nullptr) {
     constexpr bool WIN = FMT == FMT_WINDOW;
     constexpr bool OFF = FMT == FMT_OFFSET;
     constexpr bool PAT = FMT == FMT_PATTERN;
@@ -542,12 +569,13 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
             for (int u = 0; u < RU; ++u) xv[u] = p[u] ? gather_m<MODE, HALO>(a, x, c[u]) : (TX)0;
 #pragma unroll
             for (int u = 0; u < RU; ++u)
-                if (p[u]) sum[u] = (TS)v[u] * (TS)xv[u];
+                if (p[u]) sum[u] = value_of<TS>(v[u], vtab) * (TS)xv[u];
             // rows longer than L: the rest, row by row
 #pragma unroll
             for (int u = 0; u < RU; ++u)
                 for (int e = beg[u] + lane + L; e < end[u]; e += L)
-                    sum[u] = fma((TS)val_s[e - vo], (TS)gather_m<MODE, HALO>(a, x, stored_col(e)), sum[u]);
+                    sum[u] = fma(value_of<TS>(val_s[e - vo], vtab), (TS)gather_m<MODE, HALO>(a, x, stored_col(e)),
+                                 sum[u]);
 #pragma unroll
             for (int o = L / 2; o > 0; o >>= 1) {
 #pragma unroll
@@ -597,7 +625,7 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
                 //  across the gathers)
 #pragma unroll
                 for (int u = 0; u < U; ++u)
-                    if (p[u]) sum = fma((TS)val_s[e + u * L - vo], (TS)xv[u], sum);
+                    if (p[u]) sum = fma(value_of<TS>(val_s[e + u * L - vo], vtab), (TS)xv[u], sum);
             }
         }
         if (L > 1) {
@@ -619,7 +647,7 @@ __device__ __forceinline__ void compute_long(const CsrArgsT<P> &a, const BlockDe
         const int beg = __ldg(a.ptr + r), end = __ldg(a.ptr + r + 1);
         TS sum = 0;
         for (int e = beg + threadIdx.x; e < end; e += kThreads)
-            sum = fma((TS)__ldg(a.val + e), (TS)gather_m<MODE, HALO>(a, x, __ldg(a.col + e)), sum);
+            sum = fma(value_of<TS>(__ldg(a.val + e), a.vtab), (TS)gather_m<MODE, HALO>(a, x, __ldg(a.col + e)), sum);
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
         __syncthreads();                       // red_s free from the previous row
@@ -729,6 +757,10 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
     typename P::TX *win = reinterpret_cast<typename P::TX *>(stages + (size_t)nstages * lay.bytes);
     int *off_s = reinterpret_cast<int *>(stages + (size_t)nstages * lay.bytes);
     unsigned short *pstart_s = reinterpret_cast<unsigned short *>(off_s + kPatOffCap);
+    // ... and behind those an indexed operator's table of values
+    constexpr bool IDX = IndexedValues<typename P::TV>::value;
+    static_assert(!(IDX && (HALO || FMT == FMT_WINDOW)), "indexed values: single-GPU, fixed-size tables only");
+    double *vtab_s = reinterpret_cast<double *>(stages + (size_t)nstages * lay.bytes + fmt_table_bytes(FMT));
 
     const int first = blockIdx.x;
     const int step  = gridDim.x;
@@ -754,6 +786,9 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
     if constexpr (FMT == FMT_PATTERN) {
         for (int i = threadIdx.x; i < a.pat_total; i += kThreads) off_s[i] = __ldg(a.pat_off + i);
         for (int i = threadIdx.x; i <= kPatCap; i += kThreads) pstart_s[i] = __ldg(a.pat_start + i);
+    }
+    if constexpr (IDX) {
+        for (int i = threadIdx.x; i < a.vtab_n; i += kThreads) vtab_s[i] = __ldg(a.vtab + i);
     }
     __syncthreads();
     ptx::pdl_wait();         // vectors (x, f, d, y) come from earlier kernels: from here on
@@ -788,7 +823,7 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
             fill_window<MODE, HALO>(a, d, stage, lay, win);
             compute_staged<MODE, LS, HALO, P, FMT_WINDOW>(a, d, stage, lay, acc, win);
         } else if (FMT != FMT_PLAIN || (d.e1 - d.e0) <= a.nnz_cap) {
-            compute_staged<MODE, LS, HALO, P, FMT>(a, d, stage, lay, acc, nullptr, off_s, pstart_s, k0);
+            compute_staged<MODE, LS, HALO, P, FMT>(a, d, stage, lay, acc, nullptr, off_s, pstart_s, k0, vtab_s);
             k0 += (d.r1 - d.r0 + 32 / LS - 1) / (32 / LS);
         } else {
             compute_long<MODE, HALO>(a, d, red_s, acc);

@@ -13,15 +13,28 @@ namespace b200 {
 // reserved per CTA, and the kernels' static scratch (reduction + exchange tickets, < 1.5 KB)
 inline int ring_budget(int ctas) { return 228 * 1024 / ctas - 1024 - 1536; }
 
-// shared memory of one launch: header + ring of stages (+ the window / the offset table); fewer
-// stages if the configured ring does not fit beside opt_ctas_per_sm CTAs.  Returns 0 if a
-// windowed launch does not fit even with one stage.
+inline int value_table_bytes(int count) { return (count * (int)sizeof(double) + 15) & ~15; }
+
+// Does the configured ring of an operator with `count` distinct values, indexed by `idx_bytes`-byte
+// entries, keep all its stages beside the table of values?  (The index must never cost a stage.)
+// fmt: the column format the launch streams (not FMT_WINDOW).
+inline bool value_index_fits(b200_ctx_t ctx, int rows_cap, int nnz_cap, int fmt, int idx_bytes, int count) {
+    const StageLayout lay = stage_layout(rows_cap, nnz_cap, idx_bytes, fmt);
+    return fmt != FMT_WINDOW && ctx->opt_stages >= 1 &&
+           kHeaderBytes + (int)ctx->opt_stages * lay.bytes + fmt_table_bytes(fmt) + value_table_bytes(count) <=
+               ring_budget((int)ctx->opt_ctas_per_sm);
+}
+
+// shared memory of one launch: header + ring of stages (+ the window / the offset table / the
+// pattern tables, + an indexed operator's table of values); fewer stages if the configured ring
+// does not fit beside opt_ctas_per_sm CTAs.  Returns 0 if a windowed launch does not fit even with
+// one stage.
 template <class P>
 inline int ring_smem(b200_ctx_t ctx, b200_csr_t A, int fmt, int *stages_out) {
     const StageLayout lay = stage_layout(A->rows_cap, A->nnz_cap, (int)sizeof(typename P::TV), fmt, A->win_runs);
-    const int extra = fmt == FMT_WINDOW ? (int)(((size_t)A->win_slots * sizeof(typename P::TX) + 15) & ~(size_t)15)
-                      : fmt == FMT_OFFSET ? kOffTabLen * (int)sizeof(int)
-                      : fmt == FMT_PATTERN ? kPatTabBytes : 0;
+    const int extra = (fmt == FMT_WINDOW ? (int)(((size_t)A->win_slots * sizeof(typename P::TX) + 15) & ~(size_t)15)
+                                         : fmt_table_bytes(fmt)) +
+                      (IndexedValues<typename P::TV>::value ? value_table_bytes(A->vtab_n) : 0);
     int stages = (int)ctx->opt_stages;
     const int per_cta_budget = ring_budget((int)ctx->opt_ctas_per_sm);
     while (stages > 1 && kHeaderBytes + stages * lay.bytes + extra > per_cta_budget) --stages;

@@ -49,13 +49,28 @@ int b200_narrow_plan_i64(int64_t nrows, int64_t ncols, const int64_t *ptr, const
  * one-block-per-CTA variant (spmv_variant 0), the small-operator kernel and the coarse tail read
  * them.  Context option "narrow_values" (b200_ctx_set_option; env B200_NARROW_VALUES): 1 = built
  * at upload and used (default), 0 = not built / not used.
- * b200_csr_value_bytes: 4 or 8, the bytes per value the streaming passes read from A.
+ * Indexed values.  Otherwise an FP64 operator of that size whose values take at most 4,096
+ * distinct 64-bit patterns (the prolongation, restriction and first coarse operator of smoothed
+ * aggregation on a structured grid) also stores, per entry, the 8-bit (at most 256 values) or
+ * 16-bit index of its value in a table of the distinct values sorted by bit pattern; the
+ * streaming passes read 1 or 2 bytes per value and take the double from the table, the same
+ * double, so again every result keeps its bits.  Only on a single-GPU context, for an operator
+ * without long row blocks that is not windowed, and only where the table fits in shared memory
+ * beside the configured ring of stages (checked at upload and at every launch; otherwise the
+ * passes read the FP64 values).  Same option and threshold.
+ * b200_csr_value_bytes: 1, 2, 4 or 8, the bytes per value the streaming passes read from A.
  * b200_values_fit_f32: pure host helper for tests, the rule b200_csr_create applies to n values
- * (qualifies 1: every value survives the round trip). */
+ * (qualifies 1: every value survives the round trip).
+ * b200_value_index_plan_i64: pure host helper for tests, the index b200_csr_create builds from n
+ * values: width_out 8 or 16, or 0 when there are more than 4,096 distinct values (count_out is
+ * then 4097); count_out distinct values into table_out (capacity >= count_out, may be NULL);
+ * idx_out (may be NULL) receives n uint8_t (width 8) or n uint16_t (width 16). */
 int b200_csr_value_bytes(b200_csr_t A, int *bytes);
 int b200_values_fit_f32(const double *val, int64_t n, int *qualifies);
+int b200_value_index_plan_i64(const double *val, int64_t n, double *table_out, int64_t table_capacity,
+                              void *idx_out, int *count_out, int *width_out);
 
-/* b200_profile_end with the column format (B200_FMT_*) and the bytes per stored value (4 or 8)
+/* b200_profile_end with the column format (B200_FMT_*) and the bytes per stored value (1 to 8)
  * each CSR pass streamed (0 and 0 for the other kernels).  Entries are aggregated per
  * (shape, mode, format, value width). */
 typedef struct {

@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """A/B of the value width the streaming passes read (option "narrow_values": FP32 copy of an FP64
-operator whose values are all exact FP32) and of the ring shape beside it, on the real solve (one
-GPU, SA + damped Jacobi + CG on Poisson n^3).  For each option set: the solution hash against the
-first set, the solve time, and per big operator and pass the value bytes, the bytes one pass
-streams and its device time (JSON lines on stdout, the card's name and power limit first).
+operator whose values are all exact FP32, else an 8- / 16-bit index into the table of its distinct
+values) and of the ring shape beside it, on the real solve (one GPU, SA + damped Jacobi + CG on
+Poisson n^3).  For each option set: the solution hash against the first set, the solve time, and
+per big operator and pass the value bytes (1, 2, 4 or 8), the bytes one pass streams and its
+device time (JSON lines on stdout, the card's name and power limit first).
 
     python tools/values_ab.py [n] [solves] [configs]     # configs: comma-separated indices of CONFIGS
 """
