@@ -49,7 +49,7 @@ class ProfileFormatEntry(_c.Structure):
 
 
 # column formats of a CSR operator (include/amgcl_b200_formats.h B200_FMT_*)
-FORMAT_NAMES = ("plain", "window", "offset", "pattern", "col16", "col24")
+FORMAT_NAMES = ("plain", "window", "offset", "pattern", "col16", "col24", "pattern_values")
 
 
 # vecK: element-wise pass over K+1 vector streams (reads + writes)
@@ -147,6 +147,8 @@ def lib():
         "b200_ctx_largest_operator": [_vp, _P(_i64), _P(_c.c_int)],
         "b200_csr_patterns": [_vp, _P(_c.c_int), _P(_c.c_int), _P(_c.c_int)],
         "b200_pattern_plan_i64": [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _P(_c.c_int), _P(_c.c_int), _P(_c.c_int)],
+        "b200_pattern_value_plan_i64": [_i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _P(_c.c_int), _P(_c.c_int),
+                                        _P(_c.c_int), _P(_c.c_int)],
         "b200_csr_offsets": [_vp, _P(_c.c_int), _P(_c.c_int)],
         "b200_offset_plan_i64": [_i64, _i64, _vp, _vp, _vp, _vp, _P(_c.c_int), _P(_c.c_int)],
         "b200_csr_narrow": [_vp, _P(_c.c_int)],
@@ -577,7 +579,8 @@ class Csr:
     def value_bytes(self):
         """Bytes per value the streaming passes read from this operator: 4 for an FP32 operator
         and for an FP64 one whose values are all exact FP32, 1 or 2 for an FP64 one streamed as
-        indices into the table of its distinct values, else 8 (b200_csr_value_bytes)."""
+        indices into the table of its distinct values, else 8 (b200_csr_value_bytes).  For
+        value-keyed patterns, the width of the pattern table's values the passes read."""
         b = _c.c_int()
         _check(lib().b200_csr_value_bytes(self.h, _c.byref(b)))
         return b.value
@@ -611,6 +614,28 @@ def pattern_plan(nrows, ncols, ptr, col):
     if not ok.value:
         return None
     return {"pid": pid[:nrows], "start": start, "off": off, "count": cnt.value, "total": tot.value}
+
+
+def pattern_value_plan(nrows, ncols, ptr, col, val):
+    """Host-only: the value-keyed pattern format b200_csr_create tries first
+    (b200_pattern_value_plan_i64): patterns of (col - row, value) pairs.  None when the operator
+    has too many of them; else pattern_plan's fields plus "val" (the table's values, parallel to
+    "off") and "exact_f32" (every table value survives double -> float -> double)."""
+    ptr = np.ascontiguousarray(ptr, dtype=np.int64)
+    col = np.ascontiguousarray(col, dtype=np.int64)
+    val = np.ascontiguousarray(val, dtype=np.float64)
+    pid = np.zeros(max(1, nrows), dtype=np.uint8)
+    start = np.zeros(257, dtype=np.uint16)
+    off = np.zeros(1024, dtype=np.int32)
+    tab = np.zeros(1024, dtype=np.float64)
+    cnt, tot, exact, ok = _c.c_int(), _c.c_int(), _c.c_int(), _c.c_int()
+    _check(lib().b200_pattern_value_plan_i64(nrows, ncols, ptr.ctypes.data, col.ctypes.data, val.ctypes.data,
+                                             pid.ctypes.data, start.ctypes.data, off.ctypes.data, tab.ctypes.data,
+                                             _c.byref(cnt), _c.byref(tot), _c.byref(exact), _c.byref(ok)))
+    if not ok.value:
+        return None
+    return {"pid": pid[:nrows], "start": start, "off": off, "val": tab, "count": cnt.value, "total": tot.value,
+            "exact_f32": bool(exact.value)}
 
 
 def offset_plan(nrows, ncols, ptr, col):

@@ -88,6 +88,7 @@ extern "C" int b200_ctx_create(int device, b200_ctx_t *out) {
     if (const char *e = getenv("B200_POLL_SCALARS")) ctx->opt_poll_scalars = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_PATTERNS")) ctx->opt_patterns = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_PATTERNS_MIN_NNZ")) ctx->opt_patterns_min_nnz = atoll(e);
+    if (const char *e = getenv("B200_PATTERN_VALUES")) ctx->opt_pattern_values = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_OFFSETS")) ctx->opt_offsets = atoi(e) ? 1 : 0;
     if (const char *e = getenv("B200_OFFSETS_MIN_NNZ")) ctx->opt_offsets_min_nnz = atoll(e);
     if (const char *e = getenv("B200_NARROW_COLUMNS")) ctx->opt_narrow = atoi(e) ? 1 : 0;
@@ -304,6 +305,7 @@ static int64_t *option_slot(b200_ctx_t ctx, const char *key) {
     if (!strcmp(key, "small_kernel_max_nnz")) return &ctx->opt_small_kernel_max_nnz;
     if (!strcmp(key, "patterns")) return &ctx->opt_patterns;
     if (!strcmp(key, "patterns_min_nnz")) return &ctx->opt_patterns_min_nnz;
+    if (!strcmp(key, "pattern_values")) return &ctx->opt_pattern_values;
     if (!strcmp(key, "offsets")) return &ctx->opt_offsets;
     if (!strcmp(key, "offsets_min_nnz")) return &ctx->opt_offsets_min_nnz;
     if (!strcmp(key, "narrow_columns")) return &ctx->opt_narrow;

@@ -207,10 +207,17 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     }
     blk4[(size_t)nblocks] = make_int4((int)nrows, (int)nrows, (int)nnz, (int)nnz);
 
-    // ---- pattern-indexed rows, where the operator qualifies (patterns.cuh) -------------------
+    // ---- pattern-indexed rows, where the operator qualifies (patterns.cuh): keyed on the
+    // entries' values as well where those patterns fit (single GPU), else on their offsets -----
     PatternPlan patp;
-    const bool pattern_indexed = ctx->opt_patterns && nnz >= ctx->opt_patterns_min_nnz && nlong == 0 &&
-                                 lanes <= 4 && build_patterns(nrows, hptr.data(), col, patp);
+    const bool pattern_ok = ctx->opt_patterns && nnz >= ctx->opt_patterns_min_nnz && nlong == 0 && lanes <= 4;
+    const bool pattern_values = pattern_ok && ctx->opt_pattern_values && !ctx->dist &&
+                                build_patterns(nrows, hptr.data(), col, patp, val);
+    const bool pattern_indexed = pattern_values || (pattern_ok && build_patterns(nrows, hptr.data(), col, patp));
+    // ... its table also in FP32: an FP32 operator's own values, an FP64 one's where all are exact
+    const bool pattern_values32 = pattern_values &&
+        (std::is_same<Val, float>::value ||
+         (patp.val_f32 && ctx->opt_narrow_values && nnz >= ctx->opt_narrow_values_min_nnz));
 
     // ---- offset-indexed columns, where the operator qualifies (offsets.cuh) ------------------
     OffsetPlan offp;
@@ -240,9 +247,11 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
                           lanes <= 8 && build_narrow(blk4.data(), nblocks, col, nnz, nar);
 
     // ---- FP32 copy of the values of an FP64 operator that loses nothing in FP32 ----------------
+    // (not for value-keyed patterns: their passes stream no values)
     bool values32 = false;
     if constexpr (std::is_same<Val, double>::value)
-        values32 = ctx->opt_narrow_values && nnz >= ctx->opt_narrow_values_min_nnz && values_fit_f32(val, nnz);
+        values32 = !pattern_values && ctx->opt_narrow_values && nnz >= ctx->opt_narrow_values_min_nnz &&
+                   values_fit_f32(val, nnz);
 
     // ---- otherwise an index into the table of its distinct values (values.cuh), where the
     // table fits beside the configured ring of the format the operator is streamed in -----------
@@ -251,7 +260,8 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     if constexpr (std::is_same<Val, double>::value) {
         const int fmt = pattern_indexed ? FMT_PATTERN : offset_indexed ? FMT_OFFSET
                       : narrowed ? (nar.width == 24 ? FMT_COL24 : FMT_COL16) : FMT_PLAIN;
-        indexed = !values32 && ctx->opt_narrow_values && nnz > 0 && nnz >= ctx->opt_narrow_values_min_nnz &&
+        indexed = !values32 && !pattern_values && ctx->opt_narrow_values && nnz > 0 &&
+                  nnz >= ctx->opt_narrow_values_min_nnz &&
                   nlong == 0 && !windowed && !ctx->dist && build_value_index(val, nnz, vip) &&
                   value_index_fits(ctx, rows_cap, nnz_cap, fmt, vip.width / 8, vip.count);
     }
@@ -294,6 +304,8 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     const size_t tab_bytes = offset_indexed ? kOffTabLen * sizeof(int) : 0;
     const size_t pid_bytes = pattern_indexed ? (((size_t)nrows + 32 + 15) & ~(size_t)15) : 0;
     const size_t pat_bytes = pattern_indexed ? kPatOffCap * sizeof(int) + (kPatCap + 1 + 7) * sizeof(unsigned short) : 0;
+    const size_t pvl_bytes = (pattern_values ? kPatOffCap * sizeof(double) : 0) +
+                             (pattern_values32 ? kPatOffCap * sizeof(float) : 0);
     const size_t p16_bytes = ((size_t)nrows + 16) * sizeof(unsigned short);
     const size_t lo_bytes  = narrowed ? ((size_t)nnz + 16) * sizeof(unsigned short) : 0;
     const size_t hi_bytes  = narrowed && nar.width == 24 ? (((size_t)nnz + 32 + 15) & ~(size_t)15) : 0;
@@ -314,6 +326,8 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
         if (A->pid) cudaFree(A->pid);
         if (A->pat_start) cudaFree(A->pat_start);
         if (A->pat_off) cudaFree(A->pat_off);
+        if (A->pat_val) cudaFree(A->pat_val);
+        if (A->pat_val32) cudaFree(A->pat_val32);
         if (A->ptr16) cudaFree(A->ptr16);
         if (A->clo16) cudaFree(A->clo16);
         if (A->chi8) cudaFree(A->chi8);
@@ -406,10 +420,18 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
         A->pat_count = patp.count;
         A->pat_total = patp.total;
     }
+    if (pattern_values) {
+        CSR_CUDA(cudaMalloc(&A->pat_val, kPatOffCap * sizeof(double)));
+        CSR_CUDA(staged_upload(ctx, A->pat_val, patp.val.data(), (size_t)kPatOffCap));
+        if (pattern_values32) {
+            CSR_CUDA(cudaMalloc(&A->pat_val32, kPatOffCap * sizeof(float)));
+            CSR_CUDA(staged_upload(ctx, A->pat_val32, patp.val32.data(), (size_t)kPatOffCap));
+        }
+    }
     CSR_CUDA(cudaStreamSynchronize(ctx->stream));   // host staging buffers die here
 #undef CSR_CUDA
     A->bytes = ptr_bytes + col_bytes + val_bytes + v32_bytes + vix_bytes + vtb_bytes + blk_bytes + c16_bytes + run_bytes + wbk_bytes + ix8_bytes +
-               tab_bytes + pid_bytes + pat_bytes + p16_bytes + lo_bytes + hi_bytes + cb_bytes;
+               tab_bytes + pid_bytes + pat_bytes + pvl_bytes + p16_bytes + lo_bytes + hi_bytes + cb_bytes;
     if (nnz > ctx->big_nnz) {
         ctx->big_nnz = nnz;
         ctx->big_fmt = stored_format(A);
@@ -435,6 +457,8 @@ static void csr_free(b200_csr_t A) {
     if (A->pid) cudaFree(A->pid);
     if (A->pat_start) cudaFree(A->pat_start);
     if (A->pat_off) cudaFree(A->pat_off);
+    if (A->pat_val) cudaFree(A->pat_val);
+    if (A->pat_val32) cudaFree(A->pat_val32);
     if (A->ptr16) cudaFree(A->ptr16);
     if (A->clo16) cudaFree(A->clo16);
     if (A->chi8) cudaFree(A->chi8);
@@ -571,6 +595,12 @@ static int launch_csr_LH(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) 
         int rc = B200_OK;
         bool done = false;
         const int fmt = launch_format<P>(ctx, A);
+        if constexpr (L <= 4 && !HALO && !IndexedValues<typename P::TV>::value) {   // (single GPU)
+            if (fmt == FMT_PATVAL) {
+                rc = launch_ring_pv<MODE, L, P>(ctx, A, args);
+                done = true;
+            }
+        }
         if constexpr (L <= 4) {
             if (fmt == FMT_PATTERN) {
                 rc = launch_ring_pat<MODE, L, HALO, P>(ctx, A, args);
@@ -657,6 +687,16 @@ static int launch_csr(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {
         !args.gather_on && small_csr_accepts(ctx, A))
         return small_csr_launch(ctx, MODE, A, *reinterpret_cast<const CsrArgsT<PrecDD> *>(&args));
     if constexpr (std::is_same<P, PrecDD>::value) {
+        // value-keyed patterns: the FP32 table where it is exact (same doubles once widened),
+        // else the FP64 one; FMT_PATTERN streaming the FP64 values where the tables are not used
+        if (A->pat_val32 && ctx->opt_narrow_values && launch_format<PrecSD>(ctx, A) == FMT_PATVAL) {
+            CsrArgsT<PrecSD> s;
+            static_assert(sizeof(s) == sizeof(args), "PrecSD arguments differ from PrecDD only in the value type");
+            memcpy(&s, &args, sizeof(s));
+            s.val = nullptr;               // (FMT_PATVAL streams no values)
+            s.pat_val = A->pat_val32;
+            return launch_csr_lanes<MODE>(ctx, A, s);
+        }
         // the ring kernel streams the FP32 copy of an operator whose values are all exact FP32
         // (the cross-check variant, the tail and the small-operator kernel read the FP64 values)
         if (A->val32 && ctx->opt_narrow_values && ctx->opt_spmv_variant == 1) {
@@ -687,6 +727,7 @@ static CsrArgsT<P> base_args_t(b200_csr_t A) {
     a.col16 = A->col16; a.wrun = A->wrun; a.wblk = A->wblk; a.run_cap = A->win_runs;
     a.idx8 = A->idx8; a.off_tab = A->off_tab;
     a.pid = A->pid; a.pat_start = A->pat_start; a.pat_off = A->pat_off; a.pat_total = A->pat_total;
+    a.pat_val = pattern_values<typename P::TV>(A);
     a.clo16 = A->clo16; a.chi8 = A->chi8; a.cbase = A->cbase;
     return a;
 }
@@ -861,6 +902,30 @@ extern "C" int b200_pattern_plan_i64(int64_t nrows, int64_t ncols, const int64_t
     return B200_OK;
 }
 
+// The value-keyed pattern format of a host matrix (patterns.cuh), for tests.
+extern "C" int b200_pattern_value_plan_i64(int64_t nrows, int64_t ncols, const int64_t *ptr, const int64_t *col,
+                                           const double *val, uint8_t *pid_out, uint16_t *start_out,
+                                           int32_t *off_out, double *val_out, int *count, int *total,
+                                           int *exact_f32, int *qualifies) {
+    B200_REQUIRE(nrows >= 0 && ncols >= 0 && ptr && qualifies, "bad argument");
+    int rc = csr_validate(nrows, ncols, ptr, col, val != nullptr);
+    if (rc) return rc;
+    std::vector<int32_t> hptr((size_t)nrows + 1);
+    for (int64_t i = 0; i <= nrows; ++i) hptr[(size_t)i] = (int32_t)ptr[i];
+    PatternPlan o;
+    const bool ok = build_patterns(nrows, hptr.data(), col, o, val);
+    *qualifies = ok ? 1 : 0;
+    if (count) *count = ok ? o.count : 0;
+    if (total) *total = ok ? o.total : 0;
+    if (exact_f32) *exact_f32 = ok && o.val_f32 ? 1 : 0;
+    if (!ok) return B200_OK;
+    if (pid_out) std::copy(o.pid.begin(), o.pid.end(), pid_out);
+    if (start_out) std::copy(o.start.begin(), o.start.end(), start_out);
+    if (off_out) std::copy(o.off.begin(), o.off.end(), off_out);
+    if (val_out) memcpy(val_out, o.val.data(), (size_t)kPatOffCap * sizeof(double));
+    return B200_OK;
+}
+
 // The narrow column format of a host matrix (narrow.cuh), for tests: the same plan csr_upload
 // builds, without a device.  width_out: 16, 24, or 0 when the operator stays plain (a column span
 // beyond 24 bits or a long block); ptr16_out: the block-relative row pointers of that plan.
@@ -932,7 +997,7 @@ extern "C" int b200_csr_narrow(b200_csr_t A, int *width) {
 
 extern "C" int b200_csr_value_bytes(b200_csr_t A, int *bytes) {
     B200_REQUIRE(A && bytes, "null argument");
-    *bytes = A->val32 || A->dtype == B200_F32 ? 4 : A->vidx ? A->vidx_bytes : 8;
+    *bytes = A->val32 || A->pat_val32 || A->dtype == B200_F32 ? 4 : A->vidx ? A->vidx_bytes : 8;
     return B200_OK;
 }
 

@@ -163,6 +163,8 @@ struct b200_ctx_s {
     int     big_fmt = 0;                  // format it is stored in (FMT_*; for the bench's roofline)
     int64_t opt_patterns      = 1;        // operators with <= 256 distinct row patterns: no per-entry columns
     int64_t opt_patterns_min_nnz = 1000000;// ... from this many non-zeros on (decided at upload)
+    int64_t opt_pattern_values = 1;       // ... keyed on (offset, value) pairs where they fit: no per-entry
+                                          //   values or row pointers either (single GPU; patterns.cuh)
     int64_t opt_offsets       = 1;        // operators with <= 256 distinct (col - row): 8-bit column indices
     int64_t opt_offsets_min_nnz = 1000000;// ... from this many non-zeros on (decided at upload)
     int64_t opt_narrow        = 1;        // other operators: 16- or 24-bit block-relative columns (narrow.cuh)
@@ -285,6 +287,9 @@ struct b200_csr_s {
     unsigned short *pat_start = nullptr;  // [257] device
     int            *pat_off   = nullptr;  // [1024] device
     int        pat_count = 0, pat_total = 0;
+    // value-keyed patterns (FMT_PATVAL): the value of the k-th entry of row r = pat_val[pat_start[pid[r]] + k]
+    double         *pat_val   = nullptr;  // [1024] device (an FP32 operator's values widened)
+    float          *pat_val32 = nullptr;  // [1024] device, the same values as FP32 where every one is exact
     // block-relative row pointers of every staged format: ptr16[r] = ptr[r] - first non-zero of r's block
     unsigned short *ptr16 = nullptr;  // [nrows] (+ padding)
     // block-relative columns (narrow.cuh): col = cbase[block] + clo16 (+ chi8 << 16)

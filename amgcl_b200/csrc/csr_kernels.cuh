@@ -54,6 +54,13 @@
 // shared-memory load per entry, as many as the plain path needs for its staged column.  The
 // default for every operator that qualifies (the finest level of a structured-grid problem).
 //
+// Value-keyed patterns (FMT_PATVAL).  Where the pairs (offset, value) repeat as well -- a stencil
+// operator with constant coefficients, again 27 patterns for the Poisson problem -- the pattern
+// also fixes the row's values and its length: the stage holds one byte per row and nothing else,
+// and the k-th entry of row r is (col = row + off[pstart[pid] + k], value = pval[pstart[pid] + k])
+// from tables in shared memory (built by patterns.cuh).  Same entries in the same order as
+// FMT_PATTERN: the bits of the streamed values.  Single-GPU only.
+//
 // Narrow columns (FMT_COL16 / FMT_COL24).  Every other operator (no long blocks, <= 8 lanes per
 // row) stores, per block, its smallest column and, per entry, the low 16 bits of col - base, plus
 // the high 8 bits in an array of their own where some block spans more than 16 bits
@@ -88,9 +95,11 @@ enum { FMT_PLAIN = 0,     // int32 column per entry
        FMT_OFFSET = 2,    // 8-bit index into a table of (col - row) offsets
        FMT_PATTERN = 3,   // no per-entry column: 8-bit pattern id per row, col = row + pattern[k]
        FMT_COL16 = 4,     // 16-bit column relative to the block's smallest column
-       FMT_COL24 = 5 };   // the same in 24 bits: a 16-bit and an 8-bit array
+       FMT_COL24 = 5,     // the same in 24 bits: a 16-bit and an 8-bit array
+       FMT_PATVAL = 6 };  // no per-entry data: 8-bit pattern id per row, columns AND values from tables
 static_assert(FMT_PLAIN == B200_FMT_PLAIN && FMT_WINDOW == B200_FMT_WINDOW && FMT_OFFSET == B200_FMT_OFFSET &&
-              FMT_PATTERN == B200_FMT_PATTERN && FMT_COL16 == B200_FMT_COL16 && FMT_COL24 == B200_FMT_COL24,
+              FMT_PATTERN == B200_FMT_PATTERN && FMT_COL16 == B200_FMT_COL16 && FMT_COL24 == B200_FMT_COL24 &&
+              FMT_PATVAL == B200_FMT_PATVAL,
               "formats as include/amgcl_b200_formats.h reports them");
 
 enum { MODE_SPMV = 0, MODE_SPMV_ACC = 1, MODE_RESID = 2, MODE_RELAX = 3,
@@ -196,6 +205,7 @@ struct CsrArgsT {
     const unsigned short *pat_start;
     const int    *pat_off;
     int           pat_total;   // entries of pat_off in use (<= kPatOffCap)
+    const typename P::TV *pat_val;   // FMT_PATVAL: the value of every table entry, parallel to pat_off
     // Narrow columns (FMT_COL16 / FMT_COL24): col = cbase[block] + clo16[e] (+ chi8[e] << 16)
     const unsigned short *clo16;
     const unsigned char  *chi8;
@@ -224,26 +234,27 @@ __host__ __device__ inline StageLayout stage_layout(int rows_cap, int nnz_cap, i
                                                     int fmt = FMT_PLAIN, int run_cap = 0) {
     StageLayout s;
     s.val_off = 0;
-    int val_bytes = nnz_cap * val_size + 16;       // source aligned down to 16 B
+    const bool patval = fmt == FMT_PATVAL;          // (the pattern ids only)
+    int val_bytes = patval ? 0 : nnz_cap * val_size + 16;   // source aligned down to 16 B
     val_bytes = (val_bytes + 15) & ~15;
     s.col_off = s.val_off + val_bytes;
     const bool narrow = fmt == FMT_COL16 || fmt == FMT_COL24;
     int col_bytes = fmt == FMT_WINDOW || narrow ? (nnz_cap + 16) * 2   // +7 align down, +7 round up
                   : fmt == FMT_OFFSET  ? (nnz_cap + 32)       // +15 align down, +15 round up
-                  : fmt == FMT_PATTERN ? 0
+                  : fmt == FMT_PATTERN || patval ? 0
                                        : (nnz_cap + 8) * 4;   // +3 align down, +3 round up
     col_bytes = (col_bytes + 15) & ~15;
     s.hi_off = s.col_off + col_bytes;
     int hi_bytes = fmt == FMT_COL24 ? nnz_cap + 32 : 0;       // +15 align down, +15 round up
     hi_bytes = (hi_bytes + 15) & ~15;
     s.ptr_off = s.hi_off + hi_bytes;
-    int ptr_bytes = (rows_cap + 16) * 2;                      // 16-bit: +7 align down, +7 round up
+    int ptr_bytes = patval ? 0 : (rows_cap + 16) * 2;         // 16-bit: +7 align down, +7 round up
     ptr_bytes = (ptr_bytes + 15) & ~15;
     s.run_off = s.ptr_off + ptr_bytes;
     int run_bytes = fmt == FMT_WINDOW ? (run_cap + 2) * 8 : 0;   // +1 align down, +1 round up
     run_bytes = (run_bytes + 15) & ~15;
     s.pid_off = s.run_off + run_bytes;
-    int pid_bytes = fmt == FMT_PATTERN ? rows_cap + 32 : 0;      // +15 align down, +15 round up
+    int pid_bytes = fmt == FMT_PATTERN || patval ? rows_cap + 32 : 0;   // +15 align down, +15 round up
     pid_bytes = (pid_bytes + 15) & ~15;
     s.bytes = s.pid_off + pid_bytes;
     return s;
@@ -255,11 +266,12 @@ constexpr int kWinRunLen   = 64;    // longest run of a window (longer ones are 
 constexpr int kOffTabLen   = 256;   // offset-indexed operators: entries of the (col - row) table
 constexpr int kPatCap      = 256;   // pattern-indexed operators: most row patterns ...
 constexpr int kPatOffCap   = 1024;  // ... and most offsets in all patterns together
-// shared memory behind the stages: the window of x / the offset table / the pattern tables,
-// then an indexed operator's table of values
+// shared memory behind the stages: the window of x / the offset table / the pattern tables (and
+// FMT_PATVAL's values, val_size bytes each), then an indexed operator's table of values
 constexpr int kPatTabBytes = kPatOffCap * 4 + ((kPatCap + 1) * 2 + 15) / 16 * 16;
-__host__ __device__ constexpr int fmt_table_bytes(int fmt) {   // (not FMT_WINDOW: sized per operator)
-    return fmt == FMT_OFFSET ? kOffTabLen * 4 : fmt == FMT_PATTERN ? kPatTabBytes : 0;
+__host__ __device__ constexpr int fmt_table_bytes(int fmt, int val_size) {   // (not FMT_WINDOW: sized per operator)
+    return fmt == FMT_OFFSET ? kOffTabLen * 4 : fmt == FMT_PATTERN ? kPatTabBytes
+         : fmt == FMT_PATVAL ? kPatTabBytes + kPatOffCap * val_size : 0;
 }
 
 struct BlockDesc {      // written by the producer thread, read by everyone after the wait
@@ -305,10 +317,11 @@ __device__ __forceinline__ bool issue_block(const CsrArgsT<P> &a, const BlockDes
                      : "memory");
         return false;
     }
+    constexpr bool PV = FMT == FMT_PATVAL;          // (only the pattern ids)
     const int a0 = d.e0 & ~(VA - 1);
-    const int nval = ((d.e1 - a0) + VA - 1) & ~(VA - 1);
+    const int nval = PV ? 0 : ((d.e1 - a0) + VA - 1) & ~(VA - 1);
     const int p0 = d.r0 & ~7;                       // 16-bit row pointers: 8 per 16 bytes
-    const int nptr = ((d.r1 + 1 - p0) + 7) & ~7;  // (+ the next block's first row: 0)
+    const int nptr = PV ? 0 : ((d.r1 + 1 - p0) + 7) & ~7;   // (+ the next block's first row: 0)
     int ncol = 0, nhi = 0, nrun = 0, npid = 0;      // bytes of each slice
     const void *csrc = nullptr, *hsrc = nullptr, *psrc = nullptr;
     if (FMT == FMT_PLAIN) {
@@ -334,7 +347,7 @@ __device__ __forceinline__ bool issue_block(const CsrArgsT<P> &a, const BlockDes
         nrun = (((d.q1 - qa) + 1) & ~1) * 8;
         psrc = a.wrun + qa;
     }
-    if (FMT == FMT_PATTERN) {
+    if (FMT == FMT_PATTERN || PV) {
         const int q0 = d.r0 & ~15;                  // pattern ids: 16 per 16 bytes
         npid = ((d.r1 - q0) + 15) & ~15;
         psrc = a.pid + q0;
@@ -344,7 +357,7 @@ __device__ __forceinline__ bool issue_block(const CsrArgsT<P> &a, const BlockDes
     if (nval) ptx::bulk_g2s(stage + lay.val_off, a.val + a0, nval * (int)sizeof(TV), bar, policy);
     if (ncol) ptx::bulk_g2s(stage + lay.col_off, csrc, ncol, bar, policy);
     if (nhi) ptx::bulk_g2s(stage + lay.hi_off, hsrc, nhi, bar, policy);
-    ptx::bulk_g2s(stage + lay.ptr_off, a.ptr16 + p0, nptr * 2, bar, policy);
+    if (nptr) ptx::bulk_g2s(stage + lay.ptr_off, a.ptr16 + p0, nptr * 2, bar, policy);
     if (nrun) ptx::bulk_g2s(stage + lay.run_off, psrc, nrun, bar, policy);
     if (npid) ptx::bulk_g2s(stage + lay.pid_off, psrc, npid, bar, policy);
     return true;
@@ -490,6 +503,7 @@ __device__ __forceinline__ void fill_window(const CsrArgsT<P> &a, const BlockDes
 // FMT_WINDOW: x comes from the block's window, `win`, indexed by the 16-bit columns;
 // FMT_OFFSET: the column of an entry of row r is r + off[8-bit index];
 // FMT_PATTERN: the column of the k-th entry of row r is r + off[pstart[pattern id of r] + k];
+// FMT_PATVAL: the same, and its value is pval[pstart[pattern id of r] + k];
 // FMT_COL16 / FMT_COL24: the column is the block's smallest column + the stored 16 (+ 8) bits
 //
 // Rows go to warps in chunks of 32 / L rows: chunk j of the block (rows [j*32/L, (j+1)*32/L)) is
@@ -500,10 +514,12 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
                                                const char *stage, const StageLayout &lay, RowAcc &acc,
                                                const typename P::TX *win = nullptr, const int *off = nullptr,
                                                const unsigned short *pstart = nullptr, int k0 = 0,
-                                               const double *vtab = nullptr) {
+                                               const double *vtab = nullptr,
+                                               const typename P::TV *pval = nullptr) {
     constexpr bool WIN = FMT == FMT_WINDOW;
     constexpr bool OFF = FMT == FMT_OFFSET;
-    constexpr bool PAT = FMT == FMT_PATTERN;
+    constexpr bool PV  = FMT == FMT_PATVAL;
+    constexpr bool PAT = FMT == FMT_PATTERN || PV;
     constexpr bool NAR = FMT == FMT_COL16 || FMT == FMT_COL24;
     typedef typename P::TV TV;
     typedef typename P::TX TX;
@@ -595,11 +611,12 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
         if (valid) {
             // the epilogue's operands travel with the row's gathers
             if (lane == 0) ops = load_row_ops<MODE>(a, d.r0 + rr);
-            const int beg = row_beg(rr);
-            const int end = row_end(rr);
+            // PV: the row's entries are the table entries of its pattern
+            const int beg = PV ? (int)pstart[pid_s[rr]] : row_beg(rr);
+            const int end = PV ? (int)pstart[pid_s[rr] + 1] : row_end(rr);
             // PAT: the row's pattern starts at off[pb + beg], so entry e sits at off[pb + e]
             int pb = 0;
-            if (PAT) pb = (int)pstart[pid_s[rr]] - beg;
+            if (PAT && !PV) pb = (int)pstart[pid_s[rr]] - beg;
             // U independent gathers in flight per lane, then the FMAs in entry order (one lane per
             // row: short rows, a whole row of up to 8 entries goes out in one round)
             constexpr int U = (L == 1) ? 2 * kGatherBatch : kGatherBatch;
@@ -625,7 +642,7 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
                 //  across the gathers)
 #pragma unroll
                 for (int u = 0; u < U; ++u)
-                    if (p[u]) sum = fma(value_of<TS>(val_s[e + u * L - vo], vtab), (TS)xv[u], sum);
+                    if (p[u]) sum = fma(value_of<TS>(PV ? pval[e + u * L] : val_s[e + u * L - vo], vtab), (TS)xv[u], sum);
             }
         }
         if (L > 1) {
@@ -753,14 +770,19 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
     const StageLayout lay = stage_layout(a.rows_cap, a.nnz_cap, (int)sizeof(typename P::TV), FMT, a.run_cap);
     char *stages = smem + kHeaderBytes;
     // behind the stages: the window of x (FMT_WINDOW), the offset table (FMT_OFFSET), or the
-    // patterns' offsets followed by the patterns' first entries (FMT_PATTERN)
+    // patterns' offsets followed by the patterns' first entries (FMT_PATTERN) and, FMT_PATVAL,
+    // the table entries' values
     typename P::TX *win = reinterpret_cast<typename P::TX *>(stages + (size_t)nstages * lay.bytes);
     int *off_s = reinterpret_cast<int *>(stages + (size_t)nstages * lay.bytes);
     unsigned short *pstart_s = reinterpret_cast<unsigned short *>(off_s + kPatOffCap);
+    typename P::TV *pval_s = reinterpret_cast<typename P::TV *>(stages + (size_t)nstages * lay.bytes + kPatTabBytes);
     // ... and behind those an indexed operator's table of values
     constexpr bool IDX = IndexedValues<typename P::TV>::value;
-    static_assert(!(IDX && (HALO || FMT == FMT_WINDOW)), "indexed values: single-GPU, fixed-size tables only");
-    double *vtab_s = reinterpret_cast<double *>(stages + (size_t)nstages * lay.bytes + fmt_table_bytes(FMT));
+    static_assert(!(IDX && (HALO || FMT == FMT_WINDOW || FMT == FMT_PATVAL)),
+                  "indexed values: single-GPU, fixed-size tables only, values streamed");
+    static_assert(!(HALO && FMT == FMT_PATVAL), "value-keyed patterns: single-GPU only");
+    double *vtab_s = reinterpret_cast<double *>(stages + (size_t)nstages * lay.bytes +
+                                                fmt_table_bytes(FMT, (int)sizeof(typename P::TV)));
 
     const int first = blockIdx.x;
     const int step  = gridDim.x;
@@ -783,9 +805,12 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
         static_assert(kOffTabLen == kThreads, "one table entry per thread");
         off_s[threadIdx.x] = __ldg(a.off_tab + threadIdx.x);
     }
-    if constexpr (FMT == FMT_PATTERN) {
+    if constexpr (FMT == FMT_PATTERN || FMT == FMT_PATVAL) {
         for (int i = threadIdx.x; i < a.pat_total; i += kThreads) off_s[i] = __ldg(a.pat_off + i);
         for (int i = threadIdx.x; i <= kPatCap; i += kThreads) pstart_s[i] = __ldg(a.pat_start + i);
+    }
+    if constexpr (FMT == FMT_PATVAL) {
+        for (int i = threadIdx.x; i < a.pat_total; i += kThreads) pval_s[i] = __ldg(a.pat_val + i);
     }
     if constexpr (IDX) {
         for (int i = threadIdx.x; i < a.vtab_n; i += kThreads) vtab_s[i] = __ldg(a.vtab + i);
@@ -804,12 +829,13 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
     // Every warp waits on and arrives for every block, also one it has no chunk of: it reads the
     // block's descriptor, and no warp may fall a whole phase of a stage's mbarrier behind.
     // A long block (plain format) takes the whole CTA: the barriers of compute_long drain the
-    // stream up to it.  Offset- and pattern-indexed operators always run decoupled; plain and
+    // stream up to it.  Offset- and pattern-indexed operators (both pattern formats) always run decoupled; plain and
     // narrow ones where most blocks leave a warp without rows (a.row_stream, set at upload):
     // where every warp has rows anyway (the prolongation of the finest level, 256 rows of about 4
     // entries per block) the block-synchronous release measured faster.  The windowed format fills
     // its window with the whole CTA: block-synchronous.
-    const bool decoupled = FMT == FMT_OFFSET || FMT == FMT_PATTERN || (FMT != FMT_WINDOW && a.row_stream);
+    const bool decoupled = FMT == FMT_OFFSET || FMT == FMT_PATTERN || FMT == FMT_PATVAL ||
+                           (FMT != FMT_WINDOW && a.row_stream);
     constexpr int LS = FMT == FMT_PLAIN || L < 16 ? L : 8;   // (compressed formats: at most 8 lanes)
     RowAcc acc = {0.0, 0.0};
     int k0 = 0;                    // the current block's first chunk in the CTA's stream of rows
@@ -823,7 +849,7 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
             fill_window<MODE, HALO>(a, d, stage, lay, win);
             compute_staged<MODE, LS, HALO, P, FMT_WINDOW>(a, d, stage, lay, acc, win);
         } else if (FMT != FMT_PLAIN || (d.e1 - d.e0) <= a.nnz_cap) {
-            compute_staged<MODE, LS, HALO, P, FMT>(a, d, stage, lay, acc, nullptr, off_s, pstart_s, k0, vtab_s);
+            compute_staged<MODE, LS, HALO, P, FMT>(a, d, stage, lay, acc, nullptr, off_s, pstart_s, k0, vtab_s, pval_s);
             k0 += (d.r1 - d.r0 + 32 / LS - 1) / (32 / LS);
         } else {
             compute_long<MODE, HALO>(a, d, red_s, acc);

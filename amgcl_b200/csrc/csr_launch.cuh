@@ -2,7 +2,8 @@
 // api_matrices.cu (plain operators), api_window.cu (windowed operators), api_offsets.cu
 // (offset-indexed operators), api_patterns.cu (pattern-indexed operators) and api_col16.cu /
 // api_col24.cu (narrow columns): the kernel instantiations of each storage format are compiled in
-// a translation unit of their own so the build stays parallel.
+// a translation unit of their own so the build stays parallel; api_patvals.cu holds those of the
+// value-keyed pattern format.
 #pragma once
 #include "internal.cuh"
 #include "csr_kernels.cuh"
@@ -21,7 +22,7 @@ inline int value_table_bytes(int count) { return (count * (int)sizeof(double) + 
 inline bool value_index_fits(b200_ctx_t ctx, int rows_cap, int nnz_cap, int fmt, int idx_bytes, int count) {
     const StageLayout lay = stage_layout(rows_cap, nnz_cap, idx_bytes, fmt);
     return fmt != FMT_WINDOW && ctx->opt_stages >= 1 &&
-           kHeaderBytes + (int)ctx->opt_stages * lay.bytes + fmt_table_bytes(fmt) + value_table_bytes(count) <=
+           kHeaderBytes + (int)ctx->opt_stages * lay.bytes + fmt_table_bytes(fmt, idx_bytes) + value_table_bytes(count) <=
                ring_budget((int)ctx->opt_ctas_per_sm);
 }
 
@@ -33,7 +34,7 @@ template <class P>
 inline int ring_smem(b200_ctx_t ctx, b200_csr_t A, int fmt, int *stages_out) {
     const StageLayout lay = stage_layout(A->rows_cap, A->nnz_cap, (int)sizeof(typename P::TV), fmt, A->win_runs);
     const int extra = (fmt == FMT_WINDOW ? (int)(((size_t)A->win_slots * sizeof(typename P::TX) + 15) & ~(size_t)15)
-                                         : fmt_table_bytes(fmt)) +
+                                         : fmt_table_bytes(fmt, (int)sizeof(typename P::TV))) +
                       (IndexedValues<typename P::TV>::value ? value_table_bytes(A->vtab_n) : 0);
     int stages = (int)ctx->opt_stages;
     const int per_cta_budget = ring_budget((int)ctx->opt_ctas_per_sm);
@@ -74,6 +75,9 @@ int launch_ring_off(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
 // pattern-indexed operators (defined and instantiated in api_patterns.cu: 1..4 lanes per row)
 template <int MODE, int L, bool HALO, class P>
 int launch_ring_pat(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
+// value-keyed patterns (api_patvals.cu: 1..4 lanes per row, single-GPU only)
+template <int MODE, int L, class P>
+int launch_ring_pv(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
 // narrow columns (api_col16.cu / api_col24.cu: 1..8 lanes per row)
 template <int MODE, int L, bool HALO, class P>
 int launch_ring_c16(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
@@ -82,18 +86,34 @@ int launch_ring_c24(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
 
 // the column format an operator is stored in (FMT_*)
 inline int stored_format(b200_csr_t A) {
-    if (A->pid) return FMT_PATTERN;
+    if (A->pid) return A->pat_val ? FMT_PATVAL : FMT_PATTERN;
     if (A->idx8) return FMT_OFFSET;
     if (A->col16) return FMT_WINDOW;
     if (A->narrow) return A->narrow == 24 ? FMT_COL24 : FMT_COL16;
     return FMT_PLAIN;
 }
 
-// which storage format does this launch stream?
+// the table of values a value-keyed pattern operator keeps in the value type TV, or nullptr
+template <class TV>
+inline const TV *pattern_values(b200_csr_t A) {
+    if constexpr (std::is_same<TV, double>::value) return A->pat_val;
+    else if constexpr (std::is_same<TV, float>::value) return A->pat_val32;
+    else return nullptr;
+}
+
+// which storage format does this launch stream?  (FMT_PATVAL: only where the tables fit beside
+// the configured ring; options may have changed since the upload)
 template <class P>
 inline int launch_format(b200_ctx_t ctx, b200_csr_t A) {
     if (ctx->opt_spmv_variant != 1) return FMT_PLAIN;
-    if (A->pid && ctx->opt_patterns && A->lanes <= 4) return FMT_PATTERN;
+    if (A->pid && ctx->opt_patterns && A->lanes <= 4) {
+        const int vs = (int)sizeof(typename P::TV);
+        if (pattern_values<typename P::TV>(A) && ctx->opt_pattern_values && ctx->opt_stages >= 1 &&
+            kHeaderBytes + (int)ctx->opt_stages * stage_layout(A->rows_cap, A->nnz_cap, vs, FMT_PATVAL).bytes +
+                    fmt_table_bytes(FMT_PATVAL, vs) <= ring_budget((int)ctx->opt_ctas_per_sm))
+            return FMT_PATVAL;
+        return FMT_PATTERN;
+    }
     if (A->idx8 && ctx->opt_offsets && A->lanes <= 4) return FMT_OFFSET;
     if (A->col16 && ctx->opt_window && A->lanes <= 8 && A->win_runs >= 1) {
         int stages;

@@ -21,6 +21,28 @@ extern "C" {
 #define B200_FMT_PATTERN  3   /* no per-entry column: 8-bit row pattern id                  */
 #define B200_FMT_COL16    4   /* 16-bit column relative to the block's smallest column      */
 #define B200_FMT_COL24    5   /* the same in 24 bits (a 16-bit and an 8-bit array)          */
+#define B200_FMT_PATVAL   6   /* no per-entry data: 8-bit row pattern id, values in the     */
+                              /* pattern table as well                                      */
+
+/* Value-keyed patterns.  Where the pairs (col - row, value) of the rows also take at most 256
+ * patterns of at most 1024 entries in all (a stencil operator with constant coefficients: 27
+ * patterns for the 7-point Poisson problem), a single-GPU operator that qualifies for the
+ * pattern-indexed format keeps each entry's value in the pattern table too.  The streaming
+ * passes then read one byte per row and nothing per entry: the row's pattern id gives its
+ * length, columns and values.  Values are compared bit for bit (-0.0, +0.0 and NaN payloads
+ * are distinct).  The table is kept in FP64 and, where every table value is exact in FP32 and
+ * "narrow_values" applies, in FP32; the passes multiply the same doubles either way, so every
+ * result keeps its bits.  Such an operator keeps no FP32 copy and no value index.  Context
+ * option "pattern_values" (b200_ctx_set_option; env B200_PATTERN_VALUES): 1 = built at upload
+ * and used where the tables fit beside the ring of stages (default), 0 = not built / not used
+ * (the passes stream the FP64 values, format B200_FMT_PATTERN).  A pass on such an operator
+ * reports B200_FMT_PATVAL, and as value_bytes the width of the table it reads (4 or 8).
+ * b200_pattern_value_plan_i64: pure host helper for tests, the value-keyed plan b200_csr_create
+ * tries first (pid_out [nrows], start_out [257], off_out / val_out [1024]; qualifies 0: too
+ * many patterns; exact_f32 1: every table value survives double -> float -> double). */
+int b200_pattern_value_plan_i64(int64_t nrows, int64_t ncols, const int64_t *ptr, const int64_t *col,
+                                const double *val, uint8_t *pid_out, uint16_t *start_out, int32_t *off_out,
+                                double *val_out, int *count, int *total, int *exact_f32, int *qualifies);
 
 /* Narrow columns.  Inside one row block the columns of an operator span far less than the
  * int32 range.  An operator that is neither pattern- nor offset-indexed (nor windowed), has no

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """A/B of the value width the streaming passes read (option "narrow_values": FP32 copy of an FP64
 operator whose values are all exact FP32, else an 8- / 16-bit index into the table of its distinct
-values) and of the ring shape beside it, on the real solve (one GPU, SA + damped Jacobi + CG on
+values), of values kept in the pattern table (option "pattern_values": no per-entry stream at all)
+and of the ring shape beside them, on the real solve (one GPU, SA + damped Jacobi + CG on
 Poisson n^3).  For each option set: the solution hash against the first set, the solve time, and
 per big operator and pass the value bytes (1, 2, 4 or 8), the bytes one pass streams and its
 device time (JSON lines on stdout, the card's name and power limit first).
@@ -27,18 +28,24 @@ CONFIGS = [
     ("fp32 values, nnz_cap 4096", {"narrow_values": 1, "nnz_cap": 4096}),
     ("fp32 values, 3 stages", {"narrow_values": 1, "stages": 3}),
     ("fp64 values, nnz_cap 4096", {"narrow_values": 0, "nnz_cap": 4096}),
+    ("pattern values", {"pattern_values": 1}),
+    ("streamed values", {"pattern_values": 0}),
+    ("pattern values, 4 stages", {"pattern_values": 1, "stages": 4}),
 ]
-DEFAULTS = {"narrow_values": 1, "nnz_cap": 2048, "stages": 2}
+DEFAULTS = {"narrow_values": 1, "pattern_values": 1, "nnz_cap": 2048, "stages": 2}
 
 # bytes of column information per entry and of row information per row each stored format streams
-COL_BYTES = {"plain": 4, "window": 2, "offset": 1, "pattern": 0, "col16": 2, "col24": 3}
-ROW_BYTES = {"pattern": 3}      # 16-bit block-relative row pointer (+ 1 B pattern id)
+COL_BYTES = {"plain": 4, "window": 2, "offset": 1, "pattern": 0, "col16": 2, "col24": 3, "pattern_values": 0}
+ROW_BYTES = {"pattern": 3,      # 16-bit block-relative row pointer (+ 1 B pattern id)
+             "pattern_values": 1}
+VALUES_STREAMED = {"pattern_values": False}   # (values from the pattern table in shared memory)
 
 
 def streamed_bytes(p):
     """Bytes one pass moves: the stored matrix stream plus the vectors, counted as bench.py counts
     them (x once, y written, rhs / diagonal / old iterate read once per row)."""
-    b = p["nnz"] * (p["value_bytes"] + COL_BYTES[p["format"]]) + p["nrows"] * ROW_BYTES.get(p["format"], 2)
+    vb = p["value_bytes"] if VALUES_STREAMED.get(p["format"], True) else 0
+    b = p["nnz"] * (vb + COL_BYTES[p["format"]]) + p["nrows"] * ROW_BYTES.get(p["format"], 2)
     b += p["ncols"] * 8 + p["nrows"] * 8
     if p["mode"] in ("residual", "spmv_acc"):
         b += p["nrows"] * 8
