@@ -597,7 +597,7 @@ static int launch_csr_LH(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) 
         const int fmt = launch_format<P>(ctx, A);
         if constexpr (L <= 4 && !HALO && !IndexedValues<typename P::TV>::value) {   // (single GPU)
             if (fmt == FMT_PATVAL) {
-                rc = launch_ring_pv<MODE, L, P>(ctx, A, args);
+                rc = launch_patval<MODE, L, P>(ctx, A, args);
                 done = true;
             }
         }

@@ -56,10 +56,12 @@
 //
 // Value-keyed patterns (FMT_PATVAL).  Where the pairs (offset, value) repeat as well -- a stencil
 // operator with constant coefficients, again 27 patterns for the Poisson problem -- the pattern
-// also fixes the row's values and its length: the stage holds one byte per row and nothing else,
-// and the k-th entry of row r is (col = row + off[pstart[pid] + k], value = pval[pstart[pid] + k])
-// from tables in shared memory (built by patterns.cuh).  Same entries in the same order as
-// FMT_PATTERN: the bits of the streamed values.  Single-GPU only.
+// also fixes the row's values and its length: the operator streams one byte per row and nothing
+// else, and the k-th entry of row r is (col = row + off[pstart[pid] + k], value = pval[pstart[pid] + k])
+// from tables in shared memory (built by patterns.cuh).  With nothing per entry to stage, these
+// operators run csr_patval_kernel instead of the ring: it loads the ids directly and keeps several
+// rows per thread in flight.  Same entries in the same order, on the same threads, as FMT_PATTERN
+// on the ring: the bits of the streamed values.  Single-GPU only.
 //
 // Narrow columns (FMT_COL16 / FMT_COL24).  Every other operator (no long blocks, <= 8 lanes per
 // row) stores, per block, its smallest column and, per entry, the low 16 bits of col - base, plus
@@ -234,27 +236,26 @@ __host__ __device__ inline StageLayout stage_layout(int rows_cap, int nnz_cap, i
                                                     int fmt = FMT_PLAIN, int run_cap = 0) {
     StageLayout s;
     s.val_off = 0;
-    const bool patval = fmt == FMT_PATVAL;          // (the pattern ids only)
-    int val_bytes = patval ? 0 : nnz_cap * val_size + 16;   // source aligned down to 16 B
+    int val_bytes = nnz_cap * val_size + 16;        // source aligned down to 16 B
     val_bytes = (val_bytes + 15) & ~15;
     s.col_off = s.val_off + val_bytes;
     const bool narrow = fmt == FMT_COL16 || fmt == FMT_COL24;
     int col_bytes = fmt == FMT_WINDOW || narrow ? (nnz_cap + 16) * 2   // +7 align down, +7 round up
                   : fmt == FMT_OFFSET  ? (nnz_cap + 32)       // +15 align down, +15 round up
-                  : fmt == FMT_PATTERN || patval ? 0
+                  : fmt == FMT_PATTERN ? 0
                                        : (nnz_cap + 8) * 4;   // +3 align down, +3 round up
     col_bytes = (col_bytes + 15) & ~15;
     s.hi_off = s.col_off + col_bytes;
     int hi_bytes = fmt == FMT_COL24 ? nnz_cap + 32 : 0;       // +15 align down, +15 round up
     hi_bytes = (hi_bytes + 15) & ~15;
     s.ptr_off = s.hi_off + hi_bytes;
-    int ptr_bytes = patval ? 0 : (rows_cap + 16) * 2;         // 16-bit: +7 align down, +7 round up
+    int ptr_bytes = (rows_cap + 16) * 2;            // 16-bit: +7 align down, +7 round up
     ptr_bytes = (ptr_bytes + 15) & ~15;
     s.run_off = s.ptr_off + ptr_bytes;
     int run_bytes = fmt == FMT_WINDOW ? (run_cap + 2) * 8 : 0;   // +1 align down, +1 round up
     run_bytes = (run_bytes + 15) & ~15;
     s.pid_off = s.run_off + run_bytes;
-    int pid_bytes = fmt == FMT_PATTERN || patval ? rows_cap + 32 : 0;   // +15 align down, +15 round up
+    int pid_bytes = fmt == FMT_PATTERN ? rows_cap + 32 : 0;   // +15 align down, +15 round up
     pid_bytes = (pid_bytes + 15) & ~15;
     s.bytes = s.pid_off + pid_bytes;
     return s;
@@ -266,8 +267,9 @@ constexpr int kWinRunLen   = 64;    // longest run of a window (longer ones are 
 constexpr int kOffTabLen   = 256;   // offset-indexed operators: entries of the (col - row) table
 constexpr int kPatCap      = 256;   // pattern-indexed operators: most row patterns ...
 constexpr int kPatOffCap   = 1024;  // ... and most offsets in all patterns together
-// shared memory behind the stages: the window of x / the offset table / the pattern tables (and
-// FMT_PATVAL's values, val_size bytes each), then an indexed operator's table of values
+// shared memory behind the stages: the window of x / the offset table / the pattern tables, then an
+// indexed operator's table of values; FMT_PATVAL (csr_patval_kernel, no stages): the pattern tables
+// and the entries' values, val_size bytes each
 constexpr int kPatTabBytes = kPatOffCap * 4 + ((kPatCap + 1) * 2 + 15) / 16 * 16;
 __host__ __device__ constexpr int fmt_table_bytes(int fmt, int val_size) {   // (not FMT_WINDOW: sized per operator)
     return fmt == FMT_OFFSET ? kOffTabLen * 4 : fmt == FMT_PATTERN ? kPatTabBytes
@@ -317,11 +319,10 @@ __device__ __forceinline__ bool issue_block(const CsrArgsT<P> &a, const BlockDes
                      : "memory");
         return false;
     }
-    constexpr bool PV = FMT == FMT_PATVAL;          // (only the pattern ids)
     const int a0 = d.e0 & ~(VA - 1);
-    const int nval = PV ? 0 : ((d.e1 - a0) + VA - 1) & ~(VA - 1);
+    const int nval = ((d.e1 - a0) + VA - 1) & ~(VA - 1);
     const int p0 = d.r0 & ~7;                       // 16-bit row pointers: 8 per 16 bytes
-    const int nptr = PV ? 0 : ((d.r1 + 1 - p0) + 7) & ~7;   // (+ the next block's first row: 0)
+    const int nptr = ((d.r1 + 1 - p0) + 7) & ~7;    // (+ the next block's first row: 0)
     int ncol = 0, nhi = 0, nrun = 0, npid = 0;      // bytes of each slice
     const void *csrc = nullptr, *hsrc = nullptr, *psrc = nullptr;
     if (FMT == FMT_PLAIN) {
@@ -347,7 +348,7 @@ __device__ __forceinline__ bool issue_block(const CsrArgsT<P> &a, const BlockDes
         nrun = (((d.q1 - qa) + 1) & ~1) * 8;
         psrc = a.wrun + qa;
     }
-    if (FMT == FMT_PATTERN || PV) {
+    if (FMT == FMT_PATTERN) {
         const int q0 = d.r0 & ~15;                  // pattern ids: 16 per 16 bytes
         npid = ((d.r1 - q0) + 15) & ~15;
         psrc = a.pid + q0;
@@ -503,7 +504,6 @@ __device__ __forceinline__ void fill_window(const CsrArgsT<P> &a, const BlockDes
 // FMT_WINDOW: x comes from the block's window, `win`, indexed by the 16-bit columns;
 // FMT_OFFSET: the column of an entry of row r is r + off[8-bit index];
 // FMT_PATTERN: the column of the k-th entry of row r is r + off[pstart[pattern id of r] + k];
-// FMT_PATVAL: the same, and its value is pval[pstart[pattern id of r] + k];
 // FMT_COL16 / FMT_COL24: the column is the block's smallest column + the stored 16 (+ 8) bits
 //
 // Rows go to warps in chunks of 32 / L rows: chunk j of the block (rows [j*32/L, (j+1)*32/L)) is
@@ -514,12 +514,10 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
                                                const char *stage, const StageLayout &lay, RowAcc &acc,
                                                const typename P::TX *win = nullptr, const int *off = nullptr,
                                                const unsigned short *pstart = nullptr, int k0 = 0,
-                                               const double *vtab = nullptr,
-                                               const typename P::TV *pval = nullptr) {
+                                               const double *vtab = nullptr) {
     constexpr bool WIN = FMT == FMT_WINDOW;
     constexpr bool OFF = FMT == FMT_OFFSET;
-    constexpr bool PV  = FMT == FMT_PATVAL;
-    constexpr bool PAT = FMT == FMT_PATTERN || PV;
+    constexpr bool PAT = FMT == FMT_PATTERN;
     constexpr bool NAR = FMT == FMT_COL16 || FMT == FMT_COL24;
     typedef typename P::TV TV;
     typedef typename P::TX TX;
@@ -611,12 +609,11 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
         if (valid) {
             // the epilogue's operands travel with the row's gathers
             if (lane == 0) ops = load_row_ops<MODE>(a, d.r0 + rr);
-            // PV: the row's entries are the table entries of its pattern
-            const int beg = PV ? (int)pstart[pid_s[rr]] : row_beg(rr);
-            const int end = PV ? (int)pstart[pid_s[rr] + 1] : row_end(rr);
+            const int beg = row_beg(rr);
+            const int end = row_end(rr);
             // PAT: the row's pattern starts at off[pb + beg], so entry e sits at off[pb + e]
             int pb = 0;
-            if (PAT && !PV) pb = (int)pstart[pid_s[rr]] - beg;
+            if (PAT) pb = (int)pstart[pid_s[rr]] - beg;
             // U independent gathers in flight per lane, then the FMAs in entry order (one lane per
             // row: short rows, a whole row of up to 8 entries goes out in one round)
             constexpr int U = (L == 1) ? 2 * kGatherBatch : kGatherBatch;
@@ -642,7 +639,7 @@ __device__ __forceinline__ void compute_staged(const CsrArgsT<P> &a, const Block
                 //  across the gathers)
 #pragma unroll
                 for (int u = 0; u < U; ++u)
-                    if (p[u]) sum = fma(value_of<TS>(PV ? pval[e + u * L] : val_s[e + u * L - vo], vtab), (TS)xv[u], sum);
+                    if (p[u]) sum = fma(value_of<TS>(val_s[e + u * L - vo], vtab), (TS)xv[u], sum);
             }
         }
         if (L > 1) {
@@ -770,17 +767,14 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
     const StageLayout lay = stage_layout(a.rows_cap, a.nnz_cap, (int)sizeof(typename P::TV), FMT, a.run_cap);
     char *stages = smem + kHeaderBytes;
     // behind the stages: the window of x (FMT_WINDOW), the offset table (FMT_OFFSET), or the
-    // patterns' offsets followed by the patterns' first entries (FMT_PATTERN) and, FMT_PATVAL,
-    // the table entries' values
+    // patterns' offsets followed by the patterns' first entries (FMT_PATTERN)
     typename P::TX *win = reinterpret_cast<typename P::TX *>(stages + (size_t)nstages * lay.bytes);
     int *off_s = reinterpret_cast<int *>(stages + (size_t)nstages * lay.bytes);
     unsigned short *pstart_s = reinterpret_cast<unsigned short *>(off_s + kPatOffCap);
-    typename P::TV *pval_s = reinterpret_cast<typename P::TV *>(stages + (size_t)nstages * lay.bytes + kPatTabBytes);
     // ... and behind those an indexed operator's table of values
     constexpr bool IDX = IndexedValues<typename P::TV>::value;
-    static_assert(!(IDX && (HALO || FMT == FMT_WINDOW || FMT == FMT_PATVAL)),
-                  "indexed values: single-GPU, fixed-size tables only, values streamed");
-    static_assert(!(HALO && FMT == FMT_PATVAL), "value-keyed patterns: single-GPU only");
+    static_assert(FMT != FMT_PATVAL, "value-keyed patterns run csr_patval_kernel");
+    static_assert(!(IDX && (HALO || FMT == FMT_WINDOW)), "indexed values: single-GPU, fixed-size tables only");
     double *vtab_s = reinterpret_cast<double *>(stages + (size_t)nstages * lay.bytes +
                                                 fmt_table_bytes(FMT, (int)sizeof(typename P::TV)));
 
@@ -805,12 +799,9 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
         static_assert(kOffTabLen == kThreads, "one table entry per thread");
         off_s[threadIdx.x] = __ldg(a.off_tab + threadIdx.x);
     }
-    if constexpr (FMT == FMT_PATTERN || FMT == FMT_PATVAL) {
+    if constexpr (FMT == FMT_PATTERN) {
         for (int i = threadIdx.x; i < a.pat_total; i += kThreads) off_s[i] = __ldg(a.pat_off + i);
         for (int i = threadIdx.x; i <= kPatCap; i += kThreads) pstart_s[i] = __ldg(a.pat_start + i);
-    }
-    if constexpr (FMT == FMT_PATVAL) {
-        for (int i = threadIdx.x; i < a.pat_total; i += kThreads) pval_s[i] = __ldg(a.pat_val + i);
     }
     if constexpr (IDX) {
         for (int i = threadIdx.x; i < a.vtab_n; i += kThreads) vtab_s[i] = __ldg(a.vtab + i);
@@ -829,12 +820,12 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
     // Every warp waits on and arrives for every block, also one it has no chunk of: it reads the
     // block's descriptor, and no warp may fall a whole phase of a stage's mbarrier behind.
     // A long block (plain format) takes the whole CTA: the barriers of compute_long drain the
-    // stream up to it.  Offset- and pattern-indexed operators (both pattern formats) always run decoupled; plain and
+    // stream up to it.  Offset- and pattern-indexed operators always run decoupled; plain and
     // narrow ones where most blocks leave a warp without rows (a.row_stream, set at upload):
     // where every warp has rows anyway (the prolongation of the finest level, 256 rows of about 4
     // entries per block) the block-synchronous release measured faster.  The windowed format fills
     // its window with the whole CTA: block-synchronous.
-    const bool decoupled = FMT == FMT_OFFSET || FMT == FMT_PATTERN || FMT == FMT_PATVAL ||
+    const bool decoupled = FMT == FMT_OFFSET || FMT == FMT_PATTERN ||
                            (FMT != FMT_WINDOW && a.row_stream);
     constexpr int LS = FMT == FMT_PLAIN || L < 16 ? L : 8;   // (compressed formats: at most 8 lanes)
     RowAcc acc = {0.0, 0.0};
@@ -849,7 +840,7 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
             fill_window<MODE, HALO>(a, d, stage, lay, win);
             compute_staged<MODE, LS, HALO, P, FMT_WINDOW>(a, d, stage, lay, acc, win);
         } else if (FMT != FMT_PLAIN || (d.e1 - d.e0) <= a.nnz_cap) {
-            compute_staged<MODE, LS, HALO, P, FMT>(a, d, stage, lay, acc, nullptr, off_s, pstart_s, k0, vtab_s, pval_s);
+            compute_staged<MODE, LS, HALO, P, FMT>(a, d, stage, lay, acc, nullptr, off_s, pstart_s, k0, vtab_s);
             k0 += (d.r1 - d.r0 + 32 / LS - 1) / (32 / LS);
         } else {
             compute_long<MODE, HALO>(a, d, red_s, acc);
@@ -883,6 +874,151 @@ __global__ void __launch_bounds__(kThreads, 4) csr_ring_kernel(const CsrArgsT<P>
         if (++s == nstages) { s = 0; parity ^= 1; }
     }
     if (HALO && a.gather_on) gather_finish(a);
+    if (a.ndot) {
+        double v[2] = {acc.s0, acc.s1};
+        red_finish<2>(a.red, v);
+    }
+}
+
+// ---- value-keyed patterns (FMT_PATVAL): persistent CTAs without a ring ---------------------------
+// Such an operator streams one pattern id per row and nothing per entry, so there is nothing to
+// stage: each thread loads the ids of its rows itself and keeps several rows in flight.
+//
+// Same rows per thread, in the same order, as csr_ring_kernel on FMT_PATTERN (hence the same bits):
+// the same grid, CTA b walks the blocks b, b + grid, ..., chunk j of a block goes to warp (k0 + j) % 8
+// with k0 the CTA's running chunk count, and lane l of a group takes the entries l, l + L, ... of
+// its row.  A thread's rows form a software pipeline, R at a time (normally from R consecutive
+// blocks): the ids of the next batch are requested before the gathers of the current one.
+
+// rows a thread reduces together; RESID_SCALED forms every gathered value from two loads
+template <int MODE> struct PatvalBatch { static constexpr int R = MODE == MODE_RESID_SCALED ? 1 : 2; };
+
+// pattern id of a row: read once per pass, so not kept in L1 and first out of L2 (policy:
+// ptx::policy_evict_first())
+__device__ __forceinline__ int ld_pid(const unsigned char *p, uint64_t policy) {
+    unsigned v;
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u8 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(policy));
+    return (int)v;
+}
+
+template <int MODE, int L, class P>
+__global__ void __launch_bounds__(kThreads, 4) csr_patval_kernel(const CsrArgsT<P> a) {
+    typedef typename P::TV TV;
+    typedef typename P::TX TX;
+    typedef typename P::TY TS;                       // row sums live in the output's type
+    static_assert(L == 1 || L == 2 || L == 4, "value-keyed patterns: 1, 2 or 4 lanes per row");
+    static_assert(!IndexedValues<TV>::value, "value-keyed patterns keep the values themselves");
+    constexpr int R  = PatvalBatch<MODE>::R;
+    constexpr int K  = L == 1 ? 2 * kGatherBatch : kGatherBatch;   // entries per lane and row per round
+    constexpr int CR = 32 / L;                       // rows per chunk
+    constexpr int NW = kThreads / 32;
+    extern __shared__ __align__(128) char smem[];
+    int *off_s = reinterpret_cast<int *>(smem);      // the patterns' offsets,
+    unsigned short *pstart_s = reinterpret_cast<unsigned short *>(off_s + kPatOffCap);   // first entries
+    TV *pval_s = reinterpret_cast<TV *>(smem + kPatTabBytes);   // and the entries' values
+
+    const int first = blockIdx.x;
+    const int step  = gridDim.x;
+    const int mine  = (a.nblocks - first + step - 1) / step;   // blocks this CTA owns
+    const int warp  = threadIdx.x >> 5;
+    const int wl    = threadIdx.x & 31;
+    const int g     = wl / L;                        // the thread's row in a chunk
+    const int lane  = threadIdx.x % L;
+
+    // The walk.  Lane t of every warp holds the rows [r0, r1) of the CTA's blocks wb + t and
+    // wb + 32 + t, wb a multiple of 32: a block's rows come from a shuffle, and the next 32 are
+    // requested 32 blocks before they are needed.
+    auto block_rows = [&](int i) -> int2 {
+        if (i >= mine) return make_int2(0, 0);
+        const int4 q = __ldg(a.blk + first + i * step);   // (single GPU: never a halo block)
+        return make_int2(q.x, q.y);
+    };
+    int2 win_n = block_rows(wl), win_c = make_int2(0, 0);
+    int i = -1, r0 = 0, r1 = 0, k0 = 0, j = 0;       // current block, its rows, its first chunk, my next chunk
+    // this thread's next row: -1 if its group has none in the warp's next chunk, -2 at the end of
+    // the walk (both warp-uniform but the -1)
+    auto next_row = [&]() -> int {
+        while (j * CR >= r1 - r0) {                  // no chunk of the current block left for this warp
+            k0 += (r1 - r0 + CR - 1) / CR;
+            if (++i >= mine) return -2;
+            if ((i & 31) == 0) { win_c = win_n; win_n = block_rows(i + 32 + wl); }
+            r0 = __shfl_sync(0xffffffffu, win_c.x, i & 31);
+            r1 = __shfl_sync(0xffffffffu, win_c.y, i & 31);
+            j = (warp - k0) & (NW - 1);
+        }
+        const int r = r0 + j * CR + g;
+        j += NW;
+        return r < r1 ? r : -1;
+    };
+
+    // PDL: the tables and the first batch's ids are matrix data, never written by a kernel
+    const uint64_t policy = ptx::policy_evict_first();
+    for (int e = threadIdx.x; e < a.pat_total; e += kThreads) {
+        off_s[e] = __ldg(a.pat_off + e);
+        pval_s[e] = __ldg(a.pat_val + e);
+    }
+    for (int e = threadIdx.x; e <= kPatCap; e += kThreads) pstart_s[e] = __ldg(a.pat_start + e);
+    int row[R], pid[R];
+#pragma unroll
+    for (int u = 0; u < R; ++u) row[u] = next_row();
+#pragma unroll
+    for (int u = 0; u < R; ++u) pid[u] = row[u] >= 0 ? ld_pid(a.pid + row[u], policy) : 0;
+    __syncthreads();
+    ptx::pdl_wait();         // vectors (x, f, d, y) come from earlier kernels: from here on
+
+    const TX *__restrict__ x = a.x;
+    RowAcc acc = {0.0, 0.0};
+    while (row[0] != -2) {
+        // the next batch's ids travel with this batch's gathers
+        int nrow[R], npid[R];
+#pragma unroll
+        for (int u = 0; u < R; ++u) nrow[u] = next_row();
+#pragma unroll
+        for (int u = 0; u < R; ++u) npid[u] = nrow[u] >= 0 ? ld_pid(a.pid + nrow[u], policy) : 0;
+        RowOps<P> ops[R];
+        int beg[R], end[R], len = 0;
+        TS sum[R];
+#pragma unroll
+        for (int u = 0; u < R; ++u) {
+            const bool valid = row[u] >= 0;
+            ops[u] = valid && lane == 0 ? load_row_ops<MODE>(a, row[u]) : RowOps<P>{};
+            beg[u] = valid ? (int)pstart_s[pid[u]] : 0;
+            end[u] = valid ? (int)pstart_s[pid[u] + 1] : 0;
+            len = max(len, end[u] - beg[u]);
+            sum[u] = 0;
+        }
+        // K entries of every row per round, all the rows' gathers back to back, then the FMAs of
+        // each row in entry order (the values from shared memory when they are needed)
+        for (int k = lane; k < len; k += K * L) {
+            TX xv[R][K];
+#pragma unroll
+            for (int u = 0; u < R; ++u)
+#pragma unroll
+                for (int q = 0; q < K; ++q) {
+                    const int e = beg[u] + k + q * L;
+                    xv[u][q] = e < end[u] ? gather_m<MODE, false>(a, x, row[u] + off_s[e]) : (TX)0;
+                }
+#pragma unroll
+            for (int u = 0; u < R; ++u)
+#pragma unroll
+                for (int q = 0; q < K; ++q) {
+                    const int e = beg[u] + k + q * L;
+                    if (e < end[u]) sum[u] = fma((TS)pval_s[e], (TS)xv[u][q], sum[u]);
+                }
+        }
+        if (L > 1) {
+#pragma unroll
+            for (int o = L / 2; o > 0; o >>= 1) {
+#pragma unroll
+                for (int u = 0; u < R; ++u) sum[u] += __shfl_xor_sync(0xffffffffu, sum[u], o);
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < R; ++u)
+            if (row[u] >= 0 && lane == 0) store_row<MODE>(a, row[u], sum[u], acc, ops[u]);
+#pragma unroll
+        for (int u = 0; u < R; ++u) { row[u] = nrow[u]; pid[u] = npid[u]; }
+    }
     if (a.ndot) {
         double v[2] = {acc.s0, acc.s1};
         red_finish<2>(a.red, v);

@@ -2,8 +2,8 @@
 // api_matrices.cu (plain operators), api_window.cu (windowed operators), api_offsets.cu
 // (offset-indexed operators), api_patterns.cu (pattern-indexed operators) and api_col16.cu /
 // api_col24.cu (narrow columns): the kernel instantiations of each storage format are compiled in
-// a translation unit of their own so the build stays parallel; api_patvals.cu holds those of the
-// value-keyed pattern format.
+// a translation unit of their own so the build stays parallel.  Value-keyed pattern operators
+// run csr_patval_kernel instead (no ring), launched from api_patvals.cu.
 #pragma once
 #include "internal.cuh"
 #include "csr_kernels.cuh"
@@ -75,9 +75,9 @@ int launch_ring_off(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
 // pattern-indexed operators (defined and instantiated in api_patterns.cu: 1..4 lanes per row)
 template <int MODE, int L, bool HALO, class P>
 int launch_ring_pat(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
-// value-keyed patterns (api_patvals.cu: 1..4 lanes per row, single-GPU only)
+// value-keyed patterns: csr_patval_kernel, no ring (api_patvals.cu: 1..4 lanes per row, single-GPU only)
 template <int MODE, int L, class P>
-int launch_ring_pv(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
+int launch_patval(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
 // narrow columns (api_col16.cu / api_col24.cu: 1..8 lanes per row)
 template <int MODE, int L, bool HALO, class P>
 int launch_ring_c16(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
@@ -101,19 +101,12 @@ inline const TV *pattern_values(b200_csr_t A) {
     else return nullptr;
 }
 
-// which storage format does this launch stream?  (FMT_PATVAL: only where the tables fit beside
-// the configured ring; options may have changed since the upload)
+// which storage format does this launch stream?  (options may have changed since the upload)
 template <class P>
 inline int launch_format(b200_ctx_t ctx, b200_csr_t A) {
     if (ctx->opt_spmv_variant != 1) return FMT_PLAIN;
-    if (A->pid && ctx->opt_patterns && A->lanes <= 4) {
-        const int vs = (int)sizeof(typename P::TV);
-        if (pattern_values<typename P::TV>(A) && ctx->opt_pattern_values && ctx->opt_stages >= 1 &&
-            kHeaderBytes + (int)ctx->opt_stages * stage_layout(A->rows_cap, A->nnz_cap, vs, FMT_PATVAL).bytes +
-                    fmt_table_bytes(FMT_PATVAL, vs) <= ring_budget((int)ctx->opt_ctas_per_sm))
-            return FMT_PATVAL;
-        return FMT_PATTERN;
-    }
+    if (A->pid && ctx->opt_patterns && A->lanes <= 4)
+        return pattern_values<typename P::TV>(A) && ctx->opt_pattern_values ? FMT_PATVAL : FMT_PATTERN;
     if (A->idx8 && ctx->opt_offsets && A->lanes <= 4) return FMT_OFFSET;
     if (A->col16 && ctx->opt_window && A->lanes <= 8 && A->win_runs >= 1) {
         int stages;

@@ -30,7 +30,6 @@ CONFIGS = [
     ("fp64 values, nnz_cap 4096", {"narrow_values": 0, "nnz_cap": 4096}),
     ("pattern values", {"pattern_values": 1}),
     ("streamed values", {"pattern_values": 0}),
-    ("pattern values, 4 stages", {"pattern_values": 1, "stages": 4}),
 ]
 DEFAULTS = {"narrow_values": 1, "pattern_values": 1, "nnz_cap": 2048, "stages": 2}
 
