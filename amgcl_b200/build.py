@@ -101,8 +101,10 @@ def build_cuda(force=False, verbose=False):
     if failed:
         raise RuntimeError("\n".join(failed))
     objs = [os.path.join(objdir, u[:-3] + ".o") for u in units]
+    # --no-undefined: a launch the dispatcher reaches but no unit instantiates fails here, not at
+    # the first call that reaches it
     _run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-Xcompiler", "-fopenmp",
-          "-o", LIB_CUDA] + objs + ["-lgomp"])
+          "-Xlinker", "--no-undefined", "-o", LIB_CUDA] + objs + ["-lgomp"])
     return LIB_CUDA
 
 

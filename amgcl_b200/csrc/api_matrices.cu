@@ -154,6 +154,33 @@ static bool values_fit_f32(const double *val, int64_t n) {
     return !bad;
 }
 
+// One device array of operator A: `bytes` allocated and recorded in A->arrays (csr_free frees it,
+// A->bytes counts it), `count` elements of src uploaded into it as Dst, the rest (padding) zeroed.
+template <class Dst, class T, class Src>
+static cudaError_t csr_array(b200_csr_t A, T *&array, size_t bytes, const Src *src, size_t count) {
+    void *p = nullptr;
+    cudaError_t rc = cudaMalloc(&p, bytes);
+    if (rc != cudaSuccess) return rc;
+    A->arrays.emplace_back(p, bytes);
+    array = static_cast<T *>(p);
+    const size_t used = count * sizeof(Dst);
+    if (bytes > used) rc = cudaMemsetAsync(static_cast<char *>(p) + used, 0, bytes - used, A->ctx->stream);
+    if (rc == cudaSuccess && count) rc = staged_upload(A->ctx, static_cast<Dst *>(p), src, count);
+    return rc;
+}
+
+static void csr_free(b200_csr_t A) {
+    if (!A) return;
+    for (const auto &a : A->arrays) cudaFree(a.first);
+    if (A->send_idx) cudaFree(A->send_idx);
+    if (A->halo_owned) cudaFree(A->halo_owned);
+    if (A->ybuf) cudaFree(A->ybuf);
+    if (A->scratch64) cudaFree(A->scratch64);
+    if (A->pb_local) peer_release(A->ctx, A->pb_local, A->pb_peer);
+    if (A->gb_local) peer_release(A->ctx, A->gb_local, A->gb_peer);
+    delete A;
+}
+
 // Upload one CSR matrix exactly as the kernels will see it (indices narrowed to int32,
 // row-block plan built).  Single-GPU matrices come straight through here; the
 // distributed kinds hand in the local part produced by dist.cuh.
@@ -210,7 +237,8 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     // ---- pattern-indexed rows, where the operator qualifies (patterns.cuh): keyed on the
     // entries' values as well where those patterns fit (single GPU), else on their offsets -----
     PatternPlan patp;
-    const bool pattern_ok = ctx->opt_patterns && nnz >= ctx->opt_patterns_min_nnz && nlong == 0 && lanes <= 4;
+    const bool pattern_ok = ctx->opt_patterns && nnz >= ctx->opt_patterns_min_nnz && nlong == 0 &&
+                            lanes <= fmt_max_lanes(FMT_PATTERN);
     const bool pattern_values = pattern_ok && ctx->opt_pattern_values && !ctx->dist &&
                                 build_patterns(nrows, hptr.data(), col, patp, val);
     const bool pattern_indexed = pattern_values || (pattern_ok && build_patterns(nrows, hptr.data(), col, patp));
@@ -221,13 +249,14 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
 
     // ---- offset-indexed columns, where the operator qualifies (offsets.cuh) ------------------
     OffsetPlan offp;
-    const bool offset_indexed = !pattern_indexed && ctx->opt_offsets && nnz >= ctx->opt_offsets_min_nnz && nlong == 0 && lanes <= 4 &&
+    const bool offset_indexed = !pattern_indexed && ctx->opt_offsets && nnz >= ctx->opt_offsets_min_nnz && nlong == 0 &&
+                                lanes <= fmt_max_lanes(FMT_OFFSET) &&
                                 build_offsets(nrows, hptr.data(), col, offp);
 
     // ---- windowed format, where the operator qualifies (window.cuh) ------------------------
     WindowPlan win;
     bool windowed = false;
-    if (!offset_indexed && ctx->opt_window && nnz >= ctx->opt_window_min_nnz && nlong == 0 && lanes <= 8 &&
+    if (!offset_indexed && ctx->opt_window && nnz >= ctx->opt_window_min_nnz && nlong == 0 && lanes <= fmt_max_lanes(FMT_WINDOW) &&
         ((ctx->opt_window_lanes >> (lanes == 1 ? 0 : lanes == 2 ? 1 : lanes == 4 ? 2 : 3)) & 1)) {
         // what the default launch configuration leaves for the window beside two stages
         const StageLayout wl = stage_layout(rows_cap, nnz_cap, (int)sizeof(Val), FMT_WINDOW, kWinRunCapMax);
@@ -244,7 +273,7 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
     // ---- narrow columns for the operators no other format takes (narrow.cuh) -----------------
     NarrowPlan nar;
     const bool narrowed = !pattern_indexed && !offset_indexed && !windowed && ctx->opt_narrow && nlong == 0 &&
-                          lanes <= 8 && build_narrow(blk4.data(), nblocks, col, nnz, nar);
+                          lanes <= fmt_max_lanes(FMT_COL16) && build_narrow(blk4.data(), nblocks, col, nnz, nar);
 
     // ---- FP32 copy of the values of an FP64 operator that loses nothing in FP32 ----------------
     // (not for value-keyed patterns: their passes stream no values)
@@ -290,186 +319,70 @@ static int csr_upload(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
         A->row_stream = 2 * few > nblocks;
     }
     // padding: bulk copies round sizes up to 16 bytes
-    const size_t ptr_bytes = ((size_t)nrows + 1 + 8) * sizeof(int);
-    const size_t col_bytes = ((size_t)nnz + 8) * sizeof(int);
-    const size_t val_bytes = ((size_t)nnz + 8) * sizeof(Val);
-    const size_t v32_bytes = values32 ? ((size_t)nnz + 8) * sizeof(float) : 0;
-    const size_t vix_bytes = indexed ? (((size_t)nnz + 32) * (size_t)(vip.width / 8) + 15) & ~(size_t)15 : 0;
-    const size_t vtb_bytes = indexed ? (size_t)vip.count * sizeof(double) : 0;
-    const size_t blk_bytes = ((size_t)nblocks + 1) * sizeof(int4);
-    const size_t c16_bytes = windowed ? ((size_t)nnz + 16) * sizeof(unsigned short) : 0;
-    const size_t run_bytes = windowed ? (win.runs.size() + 4) * sizeof(int2) : 0;
-    const size_t wbk_bytes = windowed ? ((size_t)nblocks + 1) * sizeof(int2) : 0;
-    const size_t ix8_bytes = offset_indexed ? (((size_t)nnz + 32 + 15) & ~(size_t)15) : 0;
-    const size_t tab_bytes = offset_indexed ? kOffTabLen * sizeof(int) : 0;
-    const size_t pid_bytes = pattern_indexed ? (((size_t)nrows + 32 + 15) & ~(size_t)15) : 0;
-    const size_t pat_bytes = pattern_indexed ? kPatOffCap * sizeof(int) + (kPatCap + 1 + 7) * sizeof(unsigned short) : 0;
-    const size_t pvl_bytes = (pattern_values ? kPatOffCap * sizeof(double) : 0) +
-                             (pattern_values32 ? kPatOffCap * sizeof(float) : 0);
-    const size_t p16_bytes = ((size_t)nrows + 16) * sizeof(unsigned short);
-    const size_t lo_bytes  = narrowed ? ((size_t)nnz + 16) * sizeof(unsigned short) : 0;
-    const size_t hi_bytes  = narrowed && nar.width == 24 ? (((size_t)nnz + 32 + 15) & ~(size_t)15) : 0;
-    const size_t cb_bytes  = narrowed ? ((size_t)nblocks + 1) * sizeof(int) : 0;
-    auto cleanup = [&]() {
-        if (A->ptr) cudaFree(A->ptr);
-        if (A->col) cudaFree(A->col);
-        if (A->val) cudaFree(A->val);
-        if (A->val32) cudaFree(A->val32);
-        if (A->vidx) cudaFree(A->vidx);
-        if (A->vtab) cudaFree(A->vtab);
-        if (A->blk) cudaFree(A->blk);
-        if (A->col16) cudaFree(A->col16);
-        if (A->wrun) cudaFree(A->wrun);
-        if (A->wblk) cudaFree(A->wblk);
-        if (A->idx8) cudaFree(A->idx8);
-        if (A->off_tab) cudaFree(A->off_tab);
-        if (A->pid) cudaFree(A->pid);
-        if (A->pat_start) cudaFree(A->pat_start);
-        if (A->pat_off) cudaFree(A->pat_off);
-        if (A->pat_val) cudaFree(A->pat_val);
-        if (A->pat_val32) cudaFree(A->pat_val32);
-        if (A->ptr16) cudaFree(A->ptr16);
-        if (A->clo16) cudaFree(A->clo16);
-        if (A->chi8) cudaFree(A->chi8);
-        if (A->cbase) cudaFree(A->cbase);
-        delete A;
-    };
+    const size_t nn = (size_t)nnz, nr = (size_t)nrows, nb = (size_t)nblocks;
 #define CSR_CUDA(call)                                                         \
     do {                                                                       \
         cudaError_t rc__ = (call);                                             \
         if (rc__ != cudaSuccess) {                                             \
-            cleanup();                                                         \
+            csr_free(A);                                                       \
             return cuda_fail(rc__, #call, __FILE__, __LINE__);                 \
         }                                                                      \
     } while (0)
-    CSR_CUDA(cudaMalloc(&A->ptr, ptr_bytes));
-    CSR_CUDA(cudaMalloc(&A->col, col_bytes));
-    CSR_CUDA(cudaMalloc(&A->val, val_bytes));
-    CSR_CUDA(cudaMalloc(&A->blk, blk_bytes));
-    CSR_CUDA(cudaMemsetAsync(A->ptr, 0, ptr_bytes, ctx->stream));
-    CSR_CUDA(cudaMemsetAsync(A->col, 0, col_bytes, ctx->stream));
-    CSR_CUDA(cudaMemsetAsync(A->val, 0, val_bytes, ctx->stream));
-    CSR_CUDA(staged_upload(ctx, A->ptr, hptr.data(), (size_t)nrows + 1));
-    if (nnz) {
-        CSR_CUDA(staged_upload(ctx, A->col, col, (size_t)nnz));      // narrowed to int32 on the way
-        CSR_CUDA(staged_upload(ctx, static_cast<Val *>(A->val), val, (size_t)nnz));
-    }
-    if (values32) {
-        CSR_CUDA(cudaMalloc(&A->val32, v32_bytes));
-        CSR_CUDA(cudaMemsetAsync(A->val32, 0, v32_bytes, ctx->stream));
-        CSR_CUDA(staged_upload(ctx, A->val32, val, (size_t)nnz));     // exact: checked above
-    }
+    CSR_CUDA(csr_array<int>(A, A->ptr, (nr + 1 + 8) * sizeof(int), hptr.data(), nr + 1));
+    CSR_CUDA(csr_array<int>(A, A->col, (nn + 8) * sizeof(int), col, nn));      // narrowed to int32 on the way
+    CSR_CUDA(csr_array<Val>(A, A->val, (nn + 8) * sizeof(Val), val, nn));
+    CSR_CUDA(csr_array<int4>(A, A->blk, (nb + 1) * sizeof(int4), blk4.data(), nb + 1));
+    if (values32) CSR_CUDA(csr_array<float>(A, A->val32, (nn + 8) * sizeof(float), val, nn));   // exact: checked above
     if (indexed) {
-        CSR_CUDA(cudaMalloc(&A->vidx, vix_bytes));
-        CSR_CUDA(cudaMalloc(&A->vtab, vtb_bytes));
-        CSR_CUDA(cudaMemsetAsync(A->vidx, 0, vix_bytes, ctx->stream));
-        if (vip.width == 8) CSR_CUDA(staged_upload(ctx, static_cast<unsigned char *>(A->vidx), vip.idx8.data(), (size_t)nnz));
-        else CSR_CUDA(staged_upload(ctx, static_cast<unsigned short *>(A->vidx), vip.idx16.data(), (size_t)nnz));
-        CSR_CUDA(staged_upload(ctx, reinterpret_cast<uint64_t *>(A->vtab), vip.tab.data(), (size_t)vip.count));
+        const size_t vix_bytes = ((nn + 32) * (size_t)(vip.width / 8) + 15) & ~(size_t)15;
+        if (vip.width == 8) CSR_CUDA(csr_array<unsigned char>(A, A->vidx, vix_bytes, vip.idx8.data(), nn));
+        else CSR_CUDA(csr_array<unsigned short>(A, A->vidx, vix_bytes, vip.idx16.data(), nn));
+        CSR_CUDA(csr_array<uint64_t>(A, A->vtab, (size_t)vip.count * sizeof(double), vip.tab.data(), (size_t)vip.count));
         A->vidx_bytes = vip.width / 8;
         A->vtab_n = vip.count;
     }
-    CSR_CUDA(cudaMemcpyAsync(A->blk, blk4.data(), blk_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    CSR_CUDA(cudaMalloc(&A->ptr16, p16_bytes));
-    CSR_CUDA(cudaMemsetAsync(A->ptr16, 0, p16_bytes, ctx->stream));
-    if (nrows) CSR_CUDA(staged_upload(ctx, A->ptr16, ptr16.data(), (size_t)nrows));
+    CSR_CUDA(csr_array<unsigned short>(A, A->ptr16, (nr + 16) * sizeof(unsigned short), ptr16.data(), nr));
     if (narrowed) {
-        CSR_CUDA(cudaMalloc(&A->clo16, lo_bytes));
-        CSR_CUDA(cudaMalloc(&A->cbase, cb_bytes));
-        CSR_CUDA(cudaMemsetAsync(A->clo16, 0, lo_bytes, ctx->stream));
-        CSR_CUDA(cudaMemsetAsync(A->cbase, 0, cb_bytes, ctx->stream));
-        CSR_CUDA(staged_upload(ctx, A->clo16, nar.lo16.data(), (size_t)nnz));
-        CSR_CUDA(staged_upload(ctx, A->cbase, nar.base.data(), (size_t)nblocks));
-        if (nar.width == 24) {
-            CSR_CUDA(cudaMalloc(&A->chi8, hi_bytes));
-            CSR_CUDA(cudaMemsetAsync(A->chi8, 0, hi_bytes, ctx->stream));
-            CSR_CUDA(staged_upload(ctx, A->chi8, nar.hi8.data(), (size_t)nnz));
-        }
+        CSR_CUDA(csr_array<unsigned short>(A, A->clo16, (nn + 16) * sizeof(unsigned short), nar.lo16.data(), nn));
+        CSR_CUDA(csr_array<int>(A, A->cbase, (nb + 1) * sizeof(int), nar.base.data(), nb));
+        if (nar.width == 24)
+            CSR_CUDA(csr_array<unsigned char>(A, A->chi8, (nn + 32 + 15) & ~(size_t)15, nar.hi8.data(), nn));
         A->narrow = nar.width;
     }
     if (windowed) {
-        CSR_CUDA(cudaMalloc(&A->col16, c16_bytes));
-        CSR_CUDA(cudaMalloc(&A->wrun, run_bytes));
-        CSR_CUDA(cudaMalloc(&A->wblk, wbk_bytes));
-        CSR_CUDA(cudaMemsetAsync(A->col16, 0, c16_bytes, ctx->stream));
-        CSR_CUDA(cudaMemsetAsync(A->wrun, 0, run_bytes, ctx->stream));
-        CSR_CUDA(cudaMemsetAsync(A->wblk, 0, wbk_bytes, ctx->stream));
-        CSR_CUDA(staged_upload(ctx, A->col16, win.col16.data(), (size_t)nnz));
-        if (!win.runs.empty()) CSR_CUDA(staged_upload(ctx, A->wrun, win.runs.data(), win.runs.size()));
-        CSR_CUDA(staged_upload(ctx, A->wblk, win.wblk.data(), (size_t)nblocks));
+        CSR_CUDA(csr_array<unsigned short>(A, A->col16, (nn + 16) * sizeof(unsigned short), win.col16.data(), nn));
+        CSR_CUDA(csr_array<int2>(A, A->wrun, (win.runs.size() + 4) * sizeof(int2), win.runs.data(), win.runs.size()));
+        CSR_CUDA(csr_array<int2>(A, A->wblk, (nb + 1) * sizeof(int2), win.wblk.data(), nb));
         A->win_slots = (win.max_slots + 3) & ~3;
         A->win_runs = win.max_runs;
         A->win_total = win.total_slots;
     }
     if (offset_indexed) {
-        CSR_CUDA(cudaMalloc(&A->idx8, ix8_bytes));
-        CSR_CUDA(cudaMalloc(&A->off_tab, tab_bytes));
-        CSR_CUDA(cudaMemsetAsync(A->idx8, 0, ix8_bytes, ctx->stream));
-        CSR_CUDA(staged_upload(ctx, A->idx8, offp.idx8.data(), (size_t)nnz));
-        CSR_CUDA(staged_upload(ctx, A->off_tab, offp.tab, (size_t)kOffTabLen));
+        CSR_CUDA(csr_array<unsigned char>(A, A->idx8, (nn + 32 + 15) & ~(size_t)15, offp.idx8.data(), nn));
+        CSR_CUDA(csr_array<int>(A, A->off_tab, kOffTabLen * sizeof(int), offp.tab, (size_t)kOffTabLen));
         A->off_count = offp.count;
     }
     if (pattern_indexed) {
-        CSR_CUDA(cudaMalloc(&A->pid, pid_bytes));
-        CSR_CUDA(cudaMalloc(&A->pat_start, (kPatCap + 1 + 7) * sizeof(unsigned short)));
-        CSR_CUDA(cudaMalloc(&A->pat_off, kPatOffCap * sizeof(int)));
-        CSR_CUDA(cudaMemsetAsync(A->pid, 0, pid_bytes, ctx->stream));
-        CSR_CUDA(staged_upload(ctx, A->pid, patp.pid.data(), (size_t)nrows));
-        CSR_CUDA(staged_upload(ctx, A->pat_start, patp.start.data(), (size_t)kPatCap + 1));
-        CSR_CUDA(staged_upload(ctx, A->pat_off, patp.off.data(), (size_t)kPatOffCap));
+        CSR_CUDA(csr_array<unsigned char>(A, A->pid, (nr + 32 + 15) & ~(size_t)15, patp.pid.data(), nr));
+        CSR_CUDA(csr_array<unsigned short>(A, A->pat_start, (kPatCap + 1 + 7) * sizeof(unsigned short),
+                                           patp.start.data(), (size_t)kPatCap + 1));
+        CSR_CUDA(csr_array<int>(A, A->pat_off, kPatOffCap * sizeof(int), patp.off.data(), (size_t)kPatOffCap));
         A->pat_count = patp.count;
         A->pat_total = patp.total;
     }
-    if (pattern_values) {
-        CSR_CUDA(cudaMalloc(&A->pat_val, kPatOffCap * sizeof(double)));
-        CSR_CUDA(staged_upload(ctx, A->pat_val, patp.val.data(), (size_t)kPatOffCap));
-        if (pattern_values32) {
-            CSR_CUDA(cudaMalloc(&A->pat_val32, kPatOffCap * sizeof(float)));
-            CSR_CUDA(staged_upload(ctx, A->pat_val32, patp.val32.data(), (size_t)kPatOffCap));
-        }
-    }
+    if (pattern_values)
+        CSR_CUDA(csr_array<double>(A, A->pat_val, kPatOffCap * sizeof(double), patp.val.data(), (size_t)kPatOffCap));
+    if (pattern_values32)
+        CSR_CUDA(csr_array<float>(A, A->pat_val32, kPatOffCap * sizeof(float), patp.val32.data(), (size_t)kPatOffCap));
     CSR_CUDA(cudaStreamSynchronize(ctx->stream));   // host staging buffers die here
 #undef CSR_CUDA
-    A->bytes = ptr_bytes + col_bytes + val_bytes + v32_bytes + vix_bytes + vtb_bytes + blk_bytes + c16_bytes + run_bytes + wbk_bytes + ix8_bytes +
-               tab_bytes + pid_bytes + pat_bytes + pvl_bytes + p16_bytes + lo_bytes + hi_bytes + cb_bytes;
+    for (const auto &a : A->arrays) A->bytes += a.second;
     if (nnz > ctx->big_nnz) {
         ctx->big_nnz = nnz;
         ctx->big_fmt = stored_format(A);
     }
     *out = A;
     return B200_OK;
-}
-
-static void csr_free(b200_csr_t A) {
-    if (!A) return;
-    if (A->ptr) cudaFree(A->ptr);
-    if (A->col) cudaFree(A->col);
-    if (A->val) cudaFree(A->val);
-    if (A->val32) cudaFree(A->val32);
-    if (A->vidx) cudaFree(A->vidx);
-    if (A->vtab) cudaFree(A->vtab);
-    if (A->blk) cudaFree(A->blk);
-    if (A->col16) cudaFree(A->col16);
-    if (A->wrun) cudaFree(A->wrun);
-    if (A->wblk) cudaFree(A->wblk);
-    if (A->idx8) cudaFree(A->idx8);
-    if (A->off_tab) cudaFree(A->off_tab);
-    if (A->pid) cudaFree(A->pid);
-    if (A->pat_start) cudaFree(A->pat_start);
-    if (A->pat_off) cudaFree(A->pat_off);
-    if (A->pat_val) cudaFree(A->pat_val);
-    if (A->pat_val32) cudaFree(A->pat_val32);
-    if (A->ptr16) cudaFree(A->ptr16);
-    if (A->clo16) cudaFree(A->clo16);
-    if (A->chi8) cudaFree(A->chi8);
-    if (A->cbase) cudaFree(A->cbase);
-    if (A->send_idx) cudaFree(A->send_idx);
-    if (A->halo_owned) cudaFree(A->halo_owned);
-    if (A->ybuf) cudaFree(A->ybuf);
-    if (A->scratch64) cudaFree(A->scratch64);
-    if (A->pb_local) peer_release(A->ctx, A->pb_local, A->pb_peer);
-    if (A->gb_local) peer_release(A->ctx, A->gb_local, A->gb_peer);
-    delete A;
 }
 
 // The public constructor.  On a distributed context (dist.cuh) the shape decides how the
@@ -576,6 +489,16 @@ static int csr_create(b200_ctx_t ctx, int64_t nrows, int64_t ncols, const Ptr *p
 // P = precision combination (csr_kernels.cuh).  Only FP64 carries the multi-GPU halo path
 // and the one-block-per-CTA cross-check variant; the mixed-precision combinations use the
 // persistent ring only.
+
+// launch format FMT into rc if csr_launch.cuh's table instantiates that launch (else false)
+template <int FMT, int MODE, int L, bool HALO, class P>
+static bool launch_stored(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args, int &rc) {
+    if constexpr (!fmt_launches<FMT, L, HALO, P>()) return false;
+    else if constexpr (FMT == FMT_PATVAL) rc = launch_patval<MODE, L, P>(ctx, A, args);
+    else rc = launch_ring<FMT, MODE, L, HALO, P>(ctx, A, args);
+    return true;
+}
+
 template <int MODE, int L, bool HALO, class P>
 static int launch_csr_LH(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {
     constexpr bool fp64 = std::is_same<P, PrecDD>::value;
@@ -594,40 +517,13 @@ static int launch_csr_LH(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) 
     } else {
         int rc = B200_OK;
         bool done = false;
-        const int fmt = launch_format<P>(ctx, A);
-        if constexpr (L <= 4 && !HALO && !IndexedValues<typename P::TV>::value) {   // (single GPU)
-            if (fmt == FMT_PATVAL) {
-                rc = launch_patval<MODE, L, P>(ctx, A, args);
-                done = true;
-            }
-        }
-        if constexpr (L <= 4) {
-            if (fmt == FMT_PATTERN) {
-                rc = launch_ring_pat<MODE, L, HALO, P>(ctx, A, args);
-                done = true;
-            }
-        }
-        if constexpr (L <= 4) {
-            if (fmt == FMT_OFFSET) {
-                rc = launch_ring_off<MODE, L, HALO, P>(ctx, A, args);
-                done = true;
-            }
-        }
-        if constexpr (L <= 8 && !IndexedValues<typename P::TV>::value) {   // (indexed: never windowed)
-            if (fmt == FMT_WINDOW) {
-                rc = launch_ring_win<MODE, L, HALO, P>(ctx, A, args);
-                done = true;
-            }
-        }
-        if constexpr (L <= 8) {
-            if (fmt == FMT_COL16) {
-                rc = launch_ring_c16<MODE, L, HALO, P>(ctx, A, args);
-                done = true;
-            }
-            if (fmt == FMT_COL24) {
-                rc = launch_ring_c24<MODE, L, HALO, P>(ctx, A, args);
-                done = true;
-            }
+        switch (launch_format<P>(ctx, A)) {
+        case FMT_PATVAL:  done = launch_stored<FMT_PATVAL, MODE, L, HALO, P>(ctx, A, args, rc); break;
+        case FMT_PATTERN: done = launch_stored<FMT_PATTERN, MODE, L, HALO, P>(ctx, A, args, rc); break;
+        case FMT_OFFSET:  done = launch_stored<FMT_OFFSET, MODE, L, HALO, P>(ctx, A, args, rc); break;
+        case FMT_WINDOW:  done = launch_stored<FMT_WINDOW, MODE, L, HALO, P>(ctx, A, args, rc); break;
+        case FMT_COL16:   done = launch_stored<FMT_COL16, MODE, L, HALO, P>(ctx, A, args, rc); break;
+        case FMT_COL24:   done = launch_stored<FMT_COL24, MODE, L, HALO, P>(ctx, A, args, rc); break;
         }
         if (!done) rc = launch_ring_impl<MODE, L, HALO, P, FMT_PLAIN>(ctx, A, args);
         if (rc) return rc;
@@ -659,13 +555,21 @@ static int launch_csr_lanes(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &arg
     }
 }
 
-// the arguments of an FP64 pass, streaming A's value index instead of its values
+// the arguments of an FP64 pass streaming `val` as the values of Q (the argument layouts differ
+// only in the value type)
+template <class Q>
+static CsrArgsT<Q> retyped_args(const CsrArgsT<PrecDD> &args, const void *val) {
+    CsrArgsT<Q> s;
+    static_assert(sizeof(s) == sizeof(args), "arguments differ from PrecDD only in the value type");
+    memcpy(&s, &args, sizeof(s));
+    s.val = static_cast<const typename Q::TV *>(val);
+    return s;
+}
+
+// ... streaming A's value index into its table of values
 template <class PI>
 static CsrArgsT<PI> indexed_args(b200_csr_t A, const CsrArgsT<PrecDD> &args) {
-    CsrArgsT<PI> s;
-    static_assert(sizeof(s) == sizeof(args), "indexed arguments differ from PrecDD only in the value type");
-    memcpy(&s, &args, sizeof(s));
-    s.val = static_cast<const typename PI::TV *>(A->vidx);
+    CsrArgsT<PI> s = retyped_args<PI>(args, A->vidx);
     s.vtab = A->vtab;
     s.vtab_n = A->vtab_n;
     return s;
@@ -690,22 +594,14 @@ static int launch_csr(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {
         // value-keyed patterns: the FP32 table where it is exact (same doubles once widened),
         // else the FP64 one; FMT_PATTERN streaming the FP64 values where the tables are not used
         if (A->pat_val32 && ctx->opt_narrow_values && launch_format<PrecSD>(ctx, A) == FMT_PATVAL) {
-            CsrArgsT<PrecSD> s;
-            static_assert(sizeof(s) == sizeof(args), "PrecSD arguments differ from PrecDD only in the value type");
-            memcpy(&s, &args, sizeof(s));
-            s.val = nullptr;               // (FMT_PATVAL streams no values)
+            CsrArgsT<PrecSD> s = retyped_args<PrecSD>(args, nullptr);   // (FMT_PATVAL streams no values)
             s.pat_val = A->pat_val32;
             return launch_csr_lanes<MODE>(ctx, A, s);
         }
         // the ring kernel streams the FP32 copy of an operator whose values are all exact FP32
         // (the cross-check variant, the tail and the small-operator kernel read the FP64 values)
-        if (A->val32 && ctx->opt_narrow_values && ctx->opt_spmv_variant == 1) {
-            CsrArgsT<PrecSD> s;
-            static_assert(sizeof(s) == sizeof(args), "PrecSD arguments differ from PrecDD only in the value type");
-            memcpy(&s, &args, sizeof(s));
-            s.val = A->val32;
-            return launch_csr_lanes<MODE>(ctx, A, s);
-        }
+        if (A->val32 && ctx->opt_narrow_values && ctx->opt_spmv_variant == 1)
+            return launch_csr_lanes<MODE>(ctx, A, retyped_args<PrecSD>(args, A->val32));
         // ... or the 8- / 16-bit index of an operator with few distinct values, as long as the table
         // fits beside the configured ring (options may have changed since the upload)
         if (A->vidx && ctx->opt_narrow_values && ctx->opt_spmv_variant == 1 &&
@@ -831,7 +727,7 @@ extern "C" int b200_window_plan_i64(int64_t nrows, int64_t ncols, const int64_t 
     std::vector<int32_t> hptr((size_t)nrows + 1);
     for (int64_t i = 0; i <= nrows; ++i) hptr[(size_t)i] = (int32_t)ptr[i];
     WindowPlan w;
-    const bool ok = plan.nlong == 0 && plan.lanes <= 8 &&
+    const bool ok = plan.nlong == 0 && plan.lanes <= fmt_max_lanes(FMT_WINDOW) &&
                     build_windows(blk4.data(), nblocks, hptr.data(), col, ncols, nnz, slot_cap,
                                   kWinRunCapMax, max_ratio_percent / 100.0, gap, w);
     if (ok) {
@@ -955,7 +851,7 @@ extern "C" int b200_narrow_plan_i64(int64_t nrows, int64_t ncols, const int64_t 
         std::copy(p16.begin(), p16.end(), ptr16_out);
     }
     NarrowPlan o;
-    const bool ok = plan.nlong == 0 && plan.lanes <= 8 && build_narrow(blk4.data(), nblocks, col, nnz, o);
+    const bool ok = plan.nlong == 0 && plan.lanes <= fmt_max_lanes(FMT_COL16) && build_narrow(blk4.data(), nblocks, col, nnz, o);
     *width_out = ok ? o.width : 0;
     if (!ok) return B200_OK;
     if (base_out) {

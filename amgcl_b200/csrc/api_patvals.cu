@@ -1,6 +1,6 @@
-// api_patvals.cu -- the value-keyed pattern instantiations of the streaming CSR kernel
-// (csr_kernels.cuh, csr_patval_kernel; tables built by patterns.cuh at upload), compiled in a
-// translation unit of their own.
+// api_patvals.cu -- the value-keyed pattern launches of the streaming CSR kernel (csr_kernels.cuh,
+// csr_patval_kernel, FMT_PATVAL; tables built by patterns.cuh at upload).  A translation unit of
+// its own: the units compile concurrently.
 #include "csr_launch.cuh"
 
 namespace b200 {
@@ -16,33 +16,12 @@ int launch_patval(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {
     return B200_OK;
 }
 
-// every (mode, precision) pair api_patterns.cu instantiates except the indexed ones, for 1..4
-// lanes per row; single-GPU only, so without the multi-GPU halo
-#define B200_PV_INST(MODE, P)                                                                        \
-    template int launch_patval<MODE, 1, P>(b200_ctx_t, b200_csr_t, const CsrArgsT<P> &);             \
-    template int launch_patval<MODE, 2, P>(b200_ctx_t, b200_csr_t, const CsrArgsT<P> &);             \
-    template int launch_patval<MODE, 4, P>(b200_ctx_t, b200_csr_t, const CsrArgsT<P> &);
-
-B200_PV_INST(MODE_SPMV, PrecDD)
-B200_PV_INST(MODE_SPMV, PrecFF)
-B200_PV_INST(MODE_SPMV, PrecFD)
-B200_PV_INST(MODE_SPMV, PrecFFD)
-B200_PV_INST(MODE_SPMV_ACC, PrecDD)
-B200_PV_INST(MODE_SPMV_ACC, PrecFF)
-B200_PV_INST(MODE_SPMV_ACC, PrecFD)
-B200_PV_INST(MODE_SPMV_ACC, PrecFFD)
-B200_PV_INST(MODE_RESID, PrecDD)
-B200_PV_INST(MODE_RESID, PrecFF)
-B200_PV_INST(MODE_RESID, PrecFD)
-B200_PV_INST(MODE_RESID, PrecFDF)
-B200_PV_INST(MODE_RESID_SCALED, PrecDD)
-B200_PV_INST(MODE_RELAX, PrecDD)
-B200_PV_INST(MODE_RELAX, PrecFF)
-B200_PV_INST(MODE_RELAX, PrecFD)
-B200_PV_INST(MODE_SPMV, PrecSD)
-B200_PV_INST(MODE_SPMV_ACC, PrecSD)
-B200_PV_INST(MODE_RESID, PrecSD)
-B200_PV_INST(MODE_RESID_SCALED, PrecSD)
-B200_PV_INST(MODE_RELAX, PrecSD)
+// every pass of csr_launch.cuh's table on 1..4 lanes per row; single-GPU only, so without the
+// multi-GPU halo, and never over a value index (the tables hold the values themselves)
+static_assert(fmt_max_lanes(FMT_PATVAL) == 4 && !fmt_halo(FMT_PATVAL) && !fmt_indexed(FMT_PATVAL),
+              "the lanes, halo and indexed launches FMT_PATVAL is instantiated for");
+#define B200_PATVAL_INST(L, MODE, P) template int launch_patval<MODE, L, P>(b200_ctx_t, b200_csr_t, const CsrArgsT<P> &);
+#define B200_PATVAL_PASS(MODE, P, MAXL) B200_LANES_##MAXL(B200_PATVAL_INST, MODE, P)
+B200_CSR_PASSES(B200_PATVAL_PASS, 4)
 
 } // namespace b200

@@ -1,43 +1,7 @@
-// api_window.cu -- the windowed instantiations of the streaming CSR kernel (csr_kernels.cuh, WIN;
-// format built by window.cuh at upload).  One translation unit of their own: they double the
-// number of kernels of the library, and the units compile concurrently.
+// api_window.cu -- the windowed launches of the streaming CSR kernel (csr_kernels.cuh, FMT_WINDOW;
+// format built by window.cuh at upload): every pass of csr_launch.cuh's table on 1..8 lanes per
+// row, with and without the multi-GPU halo.  A translation unit of its own: the units compile
+// concurrently.
 #include "csr_launch.cuh"
 
-namespace b200 {
-
-template <int MODE, int L, bool HALO, class P>
-int launch_ring_win(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {
-    return launch_ring_impl<MODE, L, HALO, P, FMT_WINDOW>(ctx, A, args);
-}
-
-// every (mode, precision) pair api_matrices.cu launches, for 1..8 lanes per row, with and
-// without the multi-GPU halo
-#define B200_WIN_INST_L(MODE, L, P)                                                                  \
-    template int launch_ring_win<MODE, L, false, P>(b200_ctx_t, b200_csr_t, const CsrArgsT<P> &);    \
-    template int launch_ring_win<MODE, L, true, P>(b200_ctx_t, b200_csr_t, const CsrArgsT<P> &);
-#define B200_WIN_INST(MODE, P)                                                                       \
-    B200_WIN_INST_L(MODE, 1, P) B200_WIN_INST_L(MODE, 2, P) B200_WIN_INST_L(MODE, 4, P) B200_WIN_INST_L(MODE, 8, P)
-
-B200_WIN_INST(MODE_SPMV, PrecDD)
-B200_WIN_INST(MODE_SPMV, PrecFF)
-B200_WIN_INST(MODE_SPMV, PrecFD)
-B200_WIN_INST(MODE_SPMV, PrecFFD)
-B200_WIN_INST(MODE_SPMV_ACC, PrecDD)
-B200_WIN_INST(MODE_SPMV_ACC, PrecFF)
-B200_WIN_INST(MODE_SPMV_ACC, PrecFD)
-B200_WIN_INST(MODE_SPMV_ACC, PrecFFD)
-B200_WIN_INST(MODE_RESID, PrecDD)
-B200_WIN_INST(MODE_RESID, PrecFF)
-B200_WIN_INST(MODE_RESID, PrecFD)
-B200_WIN_INST(MODE_RESID, PrecFDF)
-B200_WIN_INST(MODE_RESID_SCALED, PrecDD)
-B200_WIN_INST(MODE_RELAX, PrecDD)
-B200_WIN_INST(MODE_RELAX, PrecFF)
-B200_WIN_INST(MODE_RELAX, PrecFD)
-B200_WIN_INST(MODE_SPMV, PrecSD)
-B200_WIN_INST(MODE_SPMV_ACC, PrecSD)
-B200_WIN_INST(MODE_RESID, PrecSD)
-B200_WIN_INST(MODE_RESID_SCALED, PrecSD)
-B200_WIN_INST(MODE_RELAX, PrecSD)
-
-} // namespace b200
+B200_RING_UNIT(FMT_WINDOW, 8, 0)

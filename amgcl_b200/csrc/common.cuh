@@ -299,6 +299,9 @@ struct b200_csr_s {
     int       *cbase    = nullptr;    // [nblocks] walk order: smallest column of the block
     int4      *blk      = nullptr;// [nblocks] device, walk order: {first row (~r if the block gathers halo
                                   //   columns), end row, first nnz, end nnz}; HALO: interior blocks first
+    // every device array above, with the bytes allocated for it (csr_array): freed by csr_free,
+    // summed into `bytes`
+    std::vector<std::pair<void *, size_t>> arrays;
     size_t     bytes    = 0;
 };
 

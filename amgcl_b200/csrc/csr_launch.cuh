@@ -1,9 +1,10 @@
-// csr_launch.cuh -- launching the persistent ring kernel (csr_kernels.cuh).  Shared by
-// api_matrices.cu (plain operators), api_window.cu (windowed operators), api_offsets.cu
-// (offset-indexed operators), api_patterns.cu (pattern-indexed operators) and api_col16.cu /
-// api_col24.cu (narrow columns): the kernel instantiations of each storage format are compiled in
-// a translation unit of their own so the build stays parallel.  Value-keyed pattern operators
-// run csr_patval_kernel instead (no ring), launched from api_patvals.cu.
+// csr_launch.cuh -- launching the persistent ring kernel (csr_kernels.cuh), and the one table of
+// the passes every column format is launched with.  api_matrices.cu launches the plain ring and
+// dispatches the other formats (launch_csr_LH); each of those formats' kernels is instantiated in
+// a translation unit of its own so the build stays parallel: api_window.cu, api_offsets.cu,
+// api_patterns.cu, api_col16.cu, api_col24.cu (launch_ring), and api_patvals.cu for the
+// value-keyed patterns' csr_patval_kernel (launch_patval, no ring).  The library is linked with
+// --no-undefined, so a launch the dispatcher reaches but no unit instantiates fails the build.
 #pragma once
 #include "internal.cuh"
 #include "csr_kernels.cuh"
@@ -66,23 +67,77 @@ inline int launch_ring_impl(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &arg
     return B200_OK;
 }
 
-// windowed operators (defined and instantiated in api_window.cu: 1..8 lanes per row)
-template <int MODE, int L, bool HALO, class P>
-int launch_ring_win(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
-// offset-indexed operators (defined and instantiated in api_offsets.cu: 1..4 lanes per row)
-template <int MODE, int L, bool HALO, class P>
-int launch_ring_off(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
-// pattern-indexed operators (defined and instantiated in api_patterns.cu: 1..4 lanes per row)
-template <int MODE, int L, bool HALO, class P>
-int launch_ring_pat(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
-// value-keyed patterns: csr_patval_kernel, no ring (api_patvals.cu: 1..4 lanes per row, single-GPU only)
+// The (MODE, Prec) pairs of every pass over an operator, each format's launches instantiated for
+// exactly these (X(MODE, P, ...) per pair) ...
+#define B200_CSR_PASSES(X, ...)                                                                      \
+    X(MODE_SPMV, PrecDD, __VA_ARGS__) X(MODE_SPMV, PrecFF, __VA_ARGS__) X(MODE_SPMV, PrecFD, __VA_ARGS__) \
+    X(MODE_SPMV, PrecFFD, __VA_ARGS__) X(MODE_SPMV, PrecSD, __VA_ARGS__)                                \
+    X(MODE_SPMV_ACC, PrecDD, __VA_ARGS__) X(MODE_SPMV_ACC, PrecFF, __VA_ARGS__)                         \
+    X(MODE_SPMV_ACC, PrecFD, __VA_ARGS__) X(MODE_SPMV_ACC, PrecFFD, __VA_ARGS__)                        \
+    X(MODE_SPMV_ACC, PrecSD, __VA_ARGS__)                                                              \
+    X(MODE_RESID, PrecDD, __VA_ARGS__) X(MODE_RESID, PrecFF, __VA_ARGS__) X(MODE_RESID, PrecFD, __VA_ARGS__) \
+    X(MODE_RESID, PrecFDF, __VA_ARGS__) X(MODE_RESID, PrecSD, __VA_ARGS__)                              \
+    X(MODE_RESID_SCALED, PrecDD, __VA_ARGS__) X(MODE_RESID_SCALED, PrecSD, __VA_ARGS__)                 \
+    X(MODE_RELAX, PrecDD, __VA_ARGS__) X(MODE_RELAX, PrecFF, __VA_ARGS__) X(MODE_RELAX, PrecFD, __VA_ARGS__) \
+    X(MODE_RELAX, PrecSD, __VA_ARGS__)
+// ... and the FP64 passes streaming an operator's value index (single-GPU only: never with the halo)
+#define B200_CSR_INDEXED_PASSES(X, ...)                                                              \
+    X(MODE_SPMV, PrecI8D, __VA_ARGS__) X(MODE_SPMV_ACC, PrecI8D, __VA_ARGS__) X(MODE_RESID, PrecI8D, __VA_ARGS__) \
+    X(MODE_RESID_SCALED, PrecI8D, __VA_ARGS__) X(MODE_RELAX, PrecI8D, __VA_ARGS__)                      \
+    X(MODE_SPMV, PrecI16D, __VA_ARGS__) X(MODE_SPMV_ACC, PrecI16D, __VA_ARGS__)                         \
+    X(MODE_RESID, PrecI16D, __VA_ARGS__) X(MODE_RESID_SCALED, PrecI16D, __VA_ARGS__)                    \
+    X(MODE_RELAX, PrecI16D, __VA_ARGS__)
+// lanes per row: 1..4 or 1..8 (X(L, ...) per lane count)
+#define B200_LANES_4(X, ...) X(1, __VA_ARGS__) X(2, __VA_ARGS__) X(4, __VA_ARGS__)
+#define B200_LANES_8(X, ...) B200_LANES_4(X, __VA_ARGS__) X(8, __VA_ARGS__)
+#define B200_IF_0(...)
+#define B200_IF_1(...) __VA_ARGS__
+
+// the most lanes per row an operator stored in a format is launched with (upload and dispatch)
+constexpr int fmt_max_lanes(int fmt) {
+    return fmt == FMT_PATTERN || fmt == FMT_OFFSET || fmt == FMT_PATVAL ? 4
+         : fmt == FMT_WINDOW || fmt == FMT_COL16 || fmt == FMT_COL24   ? 8
+                                                                       : 32;
+}
+// formats launched with the multi-GPU halo (value-keyed patterns are single-GPU only)
+constexpr bool fmt_halo(int fmt) { return fmt != FMT_PATVAL; }
+// formats launched over a value index (an indexed operator is never windowed; value-keyed patterns
+// keep the values themselves)
+constexpr bool fmt_indexed(int fmt) { return fmt != FMT_WINDOW && fmt != FMT_PATVAL; }
+// is format FMT's launch on L lanes, with or without the halo, in precision P instantiated?
+template <int FMT, int L, bool HALO, class P>
+constexpr bool fmt_launches() {
+    return L <= fmt_max_lanes(FMT) && (!HALO || fmt_halo(FMT)) &&
+           (!IndexedValues<typename P::TV>::value || fmt_indexed(FMT));
+}
+
+// the ring launches of the formats other than FMT_PLAIN and FMT_PATVAL (B200_RING_UNIT)
+template <int FMT, int MODE, int L, bool HALO, class P>
+int launch_ring(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
+// value-keyed patterns: csr_patval_kernel, no ring (api_patvals.cu)
 template <int MODE, int L, class P>
 int launch_patval(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
-// narrow columns (api_col16.cu / api_col24.cu: 1..8 lanes per row)
-template <int MODE, int L, bool HALO, class P>
-int launch_ring_c16(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
-template <int MODE, int L, bool HALO, class P>
-int launch_ring_c24(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args);
+
+// The body of one format's translation unit: defines launch_ring there only, out of
+// api_matrices.cu's view so that it instantiates no format kernel itself, and instantiates it for
+// every pass of the table on 1..MAXL lanes with and without the halo, plus, where IDX is 1, the
+// indexed passes without it.
+#define B200_RING_INST(L, FMT, MODE, P, HALO)                                                        \
+    template int launch_ring<FMT, MODE, L, HALO, P>(b200_ctx_t, b200_csr_t, const CsrArgsT<P> &);
+#define B200_RING_PASS(MODE, P, FMT, MAXL)                                                           \
+    B200_LANES_##MAXL(B200_RING_INST, FMT, MODE, P, false) B200_LANES_##MAXL(B200_RING_INST, FMT, MODE, P, true)
+#define B200_RING_INDEXED_PASS(MODE, P, FMT, MAXL) B200_LANES_##MAXL(B200_RING_INST, FMT, MODE, P, false)
+#define B200_RING_UNIT(FMT, MAXL, IDX)                                                               \
+    namespace b200 {                                                                                 \
+    static_assert(fmt_max_lanes(FMT) == MAXL && fmt_halo(FMT) && fmt_indexed(FMT) == IDX,              \
+                  "the lanes, halo and indexed launches " #FMT " is instantiated for");                \
+    template <int F, int MODE, int L, bool HALO, class P>                                            \
+    int launch_ring(b200_ctx_t ctx, b200_csr_t A, const CsrArgsT<P> &args) {                         \
+        return launch_ring_impl<MODE, L, HALO, P, F>(ctx, A, args);                                  \
+    }                                                                                                \
+    B200_CSR_PASSES(B200_RING_PASS, FMT, MAXL)                                                       \
+    B200_IF_##IDX(B200_CSR_INDEXED_PASSES(B200_RING_INDEXED_PASS, FMT, MAXL))                        \
+    }
 
 // the column format an operator is stored in (FMT_*)
 inline int stored_format(b200_csr_t A) {
@@ -105,14 +160,15 @@ inline const TV *pattern_values(b200_csr_t A) {
 template <class P>
 inline int launch_format(b200_ctx_t ctx, b200_csr_t A) {
     if (ctx->opt_spmv_variant != 1) return FMT_PLAIN;
-    if (A->pid && ctx->opt_patterns && A->lanes <= 4)
+    if (A->pid && ctx->opt_patterns && A->lanes <= fmt_max_lanes(FMT_PATTERN))
         return pattern_values<typename P::TV>(A) && ctx->opt_pattern_values ? FMT_PATVAL : FMT_PATTERN;
-    if (A->idx8 && ctx->opt_offsets && A->lanes <= 4) return FMT_OFFSET;
-    if (A->col16 && ctx->opt_window && A->lanes <= 8 && A->win_runs >= 1) {
+    if (A->idx8 && ctx->opt_offsets && A->lanes <= fmt_max_lanes(FMT_OFFSET)) return FMT_OFFSET;
+    if (A->col16 && ctx->opt_window && A->lanes <= fmt_max_lanes(FMT_WINDOW) && A->win_runs >= 1) {
         int stages;
         if (ring_smem<P>(ctx, A, FMT_WINDOW, &stages) != 0) return FMT_WINDOW;
     }
-    if (A->narrow && ctx->opt_narrow && A->lanes <= 8) return A->narrow == 24 ? FMT_COL24 : FMT_COL16;
+    if (A->narrow && ctx->opt_narrow && A->lanes <= fmt_max_lanes(A->narrow == 24 ? FMT_COL24 : FMT_COL16))
+        return A->narrow == 24 ? FMT_COL24 : FMT_COL16;
     return FMT_PLAIN;
 }
 

@@ -27,7 +27,7 @@ F64, F32 = np.float64, np.float32
 ALPHA, BETA, OMEGA = 1.5, -0.25, 0.72
 MODES = ("spmv", "spmv_acc", "resid", "relax")
 
-# (TV, TX, TF, TY, TD) and the modes each mix is launched with (api_matrices.cu, *_INST lists)
+# (TV, TX, TF, TY, TD) and the modes each mix is launched with (csr_launch.cuh, B200_CSR_PASSES)
 PRECS = {
     "DD": ((F64, F64, F64, F64, F64), MODES),
     "FD": ((F32, F64, F64, F64, F32), MODES),
